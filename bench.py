@@ -42,7 +42,33 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-pipeline", action="store_true", help="one batch at a time on one stream")
     ap.add_argument("--no-graph", action="store_true", help="do not replay the step as a CUDA graph")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    return args
+
+
+DUMP_BYTES = 64 << 20      # --dump-outputs writes at most this much in all
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each array as out_dir/<name>.npy (float32, or float64 for integer arrays, which float64 holds exactly).
+    Arrays whose rows would exceed their share of DUMP_BYTES are cut to a fixed, seeded sample of rows (sorted row
+    ids, stored beside them as <name>_rows.npy) so that two builds dump the same rows."""
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_BYTES // (2 * max(len(arrays), 1))
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float64 if a.dtype.kind in "iub" else np.float32)
+        if a.nbytes > share:
+            row_bytes = max(a.nbytes // max(a.shape[0], 1), 1)
+            keep = max(1, share // row_bytes)
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], keep, replace=False))
+            np.save(os.path.join(out_dir, name + "_rows.npy"), rows.astype(np.float64))
+            a = a[rows]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def peaks():
@@ -50,7 +76,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -241,9 +267,9 @@ def stats_ms(ts):
 
 
 def measured_traffic(key):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel from the committed `ncu --set
-    full` capture (profiles/r2_traffic.json, written by scripts/ncu_summarize.py from the .ncu-rep); null when no
-    capture of the current kernel is committed -- never a hand-copied constant."""
+    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel from a committed profiler
+    capture (profiles/r2_traffic.json); null when no capture of the current kernel is committed -- never a
+    hand-copied constant."""
     p = os.path.join(ROOT, "profiles", "r2_traffic.json")
     if not os.path.exists(p):
         return None, None
@@ -333,7 +359,7 @@ def main():
         return desc.cpu()  # ... the host gets this rank's own descriptors
 
     gathered = [None]      # the most recent all-gathered descriptor matrix (kept alive until the next step replaces it)
-    flush_buf = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)     # > 126 MB L2
+    flush_buf = torch.empty((256 << 20,), dtype=torch.uint8, device=dev)     # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -358,7 +384,7 @@ def main():
         for a, b in evs:
             flush_buf.fill_(1)            # L2 flush between timed iterations (outside the event bracket)
             a.record()
-            fn()
+            last_out[0] = fn()
             b.record()
         barrier()
         launches = (_lib.launch_count() - n0) // max(steps, 1)
@@ -463,13 +489,17 @@ def main():
         t0 = time.perf_counter()
         marks[0].record(pipe.s_enc)
         for i in range(steps):
-            one(True, marks[i + 1])
+            res = one(True, marks[i + 1])
         pipe.drain()
         barrier()
+        if last_counts[0] is not None:
+            # GraphPipeline returns the slot's capacity-sized buffer: only the last level's counts[L - 1] rows exist
+            res = res[:int(last_counts[0][len(LIMITS) - 1].item())]
+        last_out[0] = res
         wall = (time.perf_counter() - t0) * 1000.0 / steps      # synchronised on both sides
         # consecutive encoders alternate between w streams and finish in bursts: a step's time is the completion
         # interval averaged over a window of w steps (w = 1: plain consecutive intervals)
-        w = len(getattr(pipe, "s_encs", [None]))
+        w = min(len(getattr(pipe, "s_encs", [None])), steps)
         per_step = [marks[i].elapsed_time(marks[i + w]) / w for i in range(steps - w + 1)]
         launches = (_lib.launch_count() - n0) // max(steps, 1)
         if hasattr(pipe, "check"):
@@ -480,6 +510,7 @@ def main():
         return st, launches
 
     e2e_bytes = [None]
+    last_out = [None]      # what the most recent timed step returned (the descriptors of its batch)
     sampler = ClockSampler(local_rank) if rank == 0 else None
     if args.no_pipeline:
         seq, _ = timed(step_resident, args.steps, max(args.warmup, 3))      # un-pipelined latency of one batch
@@ -487,11 +518,14 @@ def main():
         seq = timed_latency(args.steps, max(args.warmup, 3))
     if args.no_pipeline:
         st, launches = timed(step_resident, args.steps, 1)
-        clocks = sampler.stop() if sampler else None
-        st_e2e, _ = timed(step_e2e, args.steps, 1)
     else:
         st, launches = timed_pipelined(args.steps, max(args.warmup, 3), False)
-        clocks = sampler.stop() if sampler else None
+    clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"descriptors": last_out[0].float().cpu().numpy()})
+    if args.no_pipeline:
+        st_e2e, _ = timed(step_e2e, args.steps, 1)
+    else:
         st_e2e, _ = timed_pipelined(args.steps, max(args.warmup, 3), True)
     # headline = the MEDIAN step (max over ranks); mean and max are reported beside it: a single host stall moves the
     # mean of 20 steps by tens of percent and says nothing about the path
@@ -682,8 +716,16 @@ def main_micro(args, world, rank, local_rank):
         return stats_ms([a.elapsed_time(b) for a, b in evs]), (_lib.launch_count() - n0) // max(steps, 1)
 
     sampler = ClockSampler(local_rank) if rank == 0 else None
-    st, launches = timed(lambda: step(P_dev), args.steps, max(args.warmup, 3))
+    last = {}
+
+    def timed_step():
+        last["out"] = step(P_dev)
+    st, launches = timed(timed_step, args.steps, max(args.warmup, 3))
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        sp_l, sb_l, nb_l = last["out"]
+        dump_outputs(args.dump_outputs, {"subsampled_points": sp_l.cpu().numpy(), "subsampled_lengths": sb_l.cpu().numpy(),
+                                         "neighbors": nb_l.cpu().numpy()})
 
     def e2e():
         sp, sb, nb = step(P_pin.to(dev, non_blocking=True))

@@ -1,4 +1,4 @@
-"""d3feat_b200 -- Blackwell-native (sm_100a) implementation of the D3Feat dense feature-extraction hot path:
+"""d3feat_b200 -- Hopper-native (sm_90a) implementation of the D3Feat dense feature-extraction hot path:
 grid subsampling -> radius neighbours -> KPConv pyramid (KPFCNN encoder), behind the reference's operator
 signatures. Host code is Python; all device code is hand-written CUDA behind the C ABI in
 include/d3feat_b200.h (d3feat_b200/libd3feat_b200.so). There is no CPU fallback."""

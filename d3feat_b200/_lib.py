@@ -61,7 +61,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise D3FError(
                 "libd3feat_b200.so is missing at %s -- build it with `python -c 'import __graft_entry__ as g; "
-                "g.build()'` (nvcc, sm_100a). d3feat_b200 has no CPU or PyTorch fallback." % LIB_PATH)
+                "g.build()'` (nvcc, sm_90a). d3feat_b200 has no CPU or PyTorch fallback." % LIB_PATH)
         l = C.CDLL(LIB_PATH)
         for name, res, args in SYMBOLS:
             fn = getattr(l, name)  # AttributeError if the .so does not export a declared symbol

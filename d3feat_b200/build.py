@@ -1,4 +1,4 @@
-"""In-tree build of libd3feat_b200.so (nvcc, sm_100a only). No JIT cache: the .so sits next to this file
+"""In-tree build of libd3feat_b200.so (nvcc, sm_90a only). No JIT cache: the .so sits next to this file
 so that it travels to the GPU box with the repository snapshot."""
 import hashlib
 import os
@@ -12,7 +12,7 @@ _STAMP = os.path.join(_HERE, "csrc", ".build_stamp")
 
 SOURCES = ["api.cu", "sort.cu", "grid.cu", "neighbors.cu", "kpconv.cu", "kpconv_fused.cu", "gemm.cu", "pool.cu", "tc_gemm.cu", "pyramid.cu"]
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]
 
 
@@ -36,7 +36,7 @@ def _digest():
 
 
 def build(force=False, verbose=False):
-    """Compile every .cu for sm_100a and link the shared library. Returns the path of the .so."""
+    """Compile every .cu for sm_90a and link the shared library. Returns the path of the .so."""
     srcs = [s for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
     dig = _digest()
     if not force and os.path.exists(LIB) and os.path.exists(_STAMP) and open(_STAMP).read().strip() == dig:

@@ -1,5 +1,5 @@
 """Mirror of kernels/convolution_ops.py: same function names, argument order and error behaviour, backed by
-the fused sm_100a KPConv kernels through the C ABI (include/d3feat_b200.h).
+the fused sm_90a KPConv kernels through the C ABI (include/d3feat_b200.h).
 
   unary_convolution(features, K_values)                                   convolution_ops.py:90-99
   KPConv(query_points, support_points, neighbors_indices, features, K_values, fixed='center',
@@ -27,7 +27,7 @@ from . import _lib
 from . import variables as V
 
 # Tensor-core path: static weights are packed once per weight tensor into the K-major TF32 hi/lo images the
-# tcgen05 kernels consume (d3f_pack_weight). D3F_TENSOR_CORES=0 selects the CUDA-core fp32 kernels instead.
+# wgmma kernels consume (d3f_pack_weight). D3F_TENSOR_CORES=0 selects the CUDA-core fp32 kernels instead.
 USE_TENSOR_CORES = os.environ.get("D3F_TENSOR_CORES", "1") != "0"
 _packed_cache = {}     # id(tensor) -> (weakref, version, packed image); entries die with their tensor
 

@@ -1,4 +1,4 @@
-// Shared helpers for the d3feat_b200 CUDA library (sm_100a only).
+// Shared helpers for the d3feat_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -34,7 +34,7 @@ void count_launch(int n = 1);
     }                                \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM
 constexpr int kMaxBatch = 1024;
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }

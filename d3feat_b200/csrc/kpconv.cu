@@ -12,7 +12,7 @@
 //   kpconv_cin1_kernel<FAST>         first layer (Cin = 1), whole operator in one kernel
 //   kpconv_stage1_anyk_kernel, _v2_kernel, _kernel   CUDA-core paths: any number of kernel points, odd widths
 // Stage 2 is the dense contraction  out[n,:] = (sum_k wf[n,k,:] @ W[k]) / nn[n]  ==  [Nq, K*Cin] @ [K*Cin, Cout] on
-// tcgen05 with the block epilogue fused (tc_gemm.cu; gemm.cu without tensor cores). The [N,H,K,3], [N,H,K], [N,H,Cin]
+// wgmma with the block epilogue fused (tc_gemm.cu; gemm.cu without tensor cores). The [N,H,K,3], [N,H,K], [N,H,Cin]
 // intermediates of the TF graph are never materialised; wf is one buffer per layer (chunks beyond 512 MB).
 // kpconv_fused.cu holds the single persistent kernel (stage 1 + contraction) for the Cin = Cout = 32 layers (opt-in).
 #include <stdlib.h>
@@ -248,16 +248,13 @@ __global__ void __launch_bounds__(kS1Warps * 32) kpconv_stage1_kernel(Stage1Para
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Stage 1, packed-FMA version (the one the encoder's layers use). Blackwell reaches its full fp32 rate only
-// through FFMA2 (fma.rn.f32x2): the K = 15 kernel points are padded to 16 and handled as 8 PAIRS, so one
-// FFMA2 updates (wf[2j], wf[2j+1]) of a channel: 8 FFMA2 per neighbour and channel instead of 15 FFMA, fed by
-// four broadcast LDS.128 that deliver the pairs already packed. For Cin = 32 a warp serves TWO queries (one
-// per half-warp, 2 channels per lane) so that the weight reads and the row loads are amortised over both.
+// Stage 1, paired-kernel-point version (the one the encoder's layers use): the K = 15 kernel points are padded to 16
+// and handled as 8 PAIRS, so one ffma2 updates (wf[2j], wf[2j+1]) of a channel, fed by four broadcast LDS.128 that
+// deliver the pairs already packed. For Cin = 32 a warp serves TWO queries (one per half-warp, 2 channels per lane) so
+// that the weight reads and the row loads are amortised over both.
+// sm_90 has no packed fp32 FMA: a pair is two FFMA with the same round-to-nearest result per element.
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  unsigned long long ra = *reinterpret_cast<unsigned long long*>(&a), rb = *reinterpret_cast<unsigned long long*>(&b),
-                     rc = *reinterpret_cast<unsigned long long*>(&c), rd;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-  return *reinterpret_cast<float2*>(&rd);
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
 
 // MUFU.SQRT: one instruction instead of the ~10-instruction IEEE sequence (max error ~1 ulp; tolerance 1e-4). The
@@ -411,8 +408,8 @@ __global__ void __launch_bounds__(kS1Warps * 32, CPL == 4 ? 4 : 6) kpconv_stage1
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Stage 1 on the tensor pipe (warp-level mma.sync.m16n8k8 TF32, 3xTF32 split; measured 277 TFLOP/s on B200 =
-// 3.8x the FFMA2 fp32 peak, scripts/micro/mma_sync_rate.cu). Per query and 8-neighbour step:
+// Stage 1 on the tensor pipe (warp-level mma.sync.m16n8k8 TF32, 3xTF32 split: even three TF32 products per fp32 one
+// run well above the CUDA-core fp32 rate). Per query and 8-neighbour step:
 //     wf[16 kernel pts, channels] += W^T[16 x 8 neighbours] . F[8 neighbours x channels]
 // * A (correlation weights) is computed DIRECTLY in fragment layout: lane (g = lane/4, t = lane%4) evaluates the
 //   weights of neighbours {8s+t, 8s+t+4} against kernel points {g, g+8} -- they live in registers, no shared memory.
@@ -432,9 +429,8 @@ __device__ __forceinline__ void split3(float x, unsigned& hi, unsigned& lo) {
 
 // ---------------------------------------------------------------------------------------------------
 // The same stage 1 with the instruction stream pared down for the configuration every D3Feat model runs (rigid, linear
-// influence, sum aggregation). ncu (profiles/r2_all_kernels_ncu.txt) shows the general kernel issue
-// bound at 63 % with ~190 instructions per 8-neighbour step, of which barely 90 are the correlation / split / MMA
-// work. What is removed here:
+// influence, sum aggregation). The general kernel is issue bound, and less than half of its instructions per
+// 8-neighbour step are the correlation / split / MMA work. What is removed here:
 //  * the shadow test on the weights: the rigid shadow point sits at 1e6 (:190), its linear influence is
 //    max(1 - ~1e7, 0) = 0 on its own; the same trick parks the 16th (non-existent) kernel point of lanes g = 7 at 1e6;
 //  * the ballot / popc chain of the neighbour count: every lane counts its own two neighbours, lanes 0-3 are reduced
@@ -543,8 +539,8 @@ kpconv_stage1_fast_kernel(Stage1Params p) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-// The pared kernel with the gathers STAGED through shared memory. ncu of the kernel above (profiles/r2_stage1_ncu.txt):
-// the L1 data pipe is the bound (l1tex__data_pipe_lsu_wavefronts 88 % of peak) -- a 128-bit warp load is served a
+// The pared kernel with the gathers STAGED through shared memory. The kernel above can be bound by the L1 data pipe
+// (LSU wavefronts) -- a 128-bit warp load is served a
 // quarter-warp at a time, one wavefront per cache line the quarter touches, and in the mma fragment layout
 // (lane = 4 g + t, neighbour <-> t) every quarter holds four neighbours: 16 wavefronts per row load instead of 4, and
 // the same for the packed points. Here the rows of a step arrive by cp.async in the COALESCED assignment (the 8 lanes
@@ -1132,16 +1128,10 @@ static AuxStream* aux_stream() {
 }
 
 // Queries per chunk of the two-kernel path (stage 1 writes wf[chunk, K*Cin], the contraction of chunk i overlaps
-// stage 1 of chunk i+1). Measured on B200 (profiles/r2_notes.md, 8 x 30k fragments, warm):
-//     rows per chunk       32->32 @ 240k   64->64 @ 60k   128->128 @ 15k
-//     40 MB of wf (r1)        0.60 ms         0.40 ms         0.20 ms
-//     37 888                  0.60            0.27            0.16
-//     75 776 / 120 064        0.56 / 0.57     0.26            0.16
-//     the whole layer         0.54            0.26            0.16
-// Keeping a chunk inside the 126 MB L2 is NOT what matters: every chunk costs a stage-1 tail, a GEMM launch with its
-// fixed latency and a partial wave, and both kernels fill the machine on their own so the overlap buys little, while
-// HBM takes the 460 MB wf round trip of the largest layer in well under the stage-1 time. So: one chunk per layer
-// up to 512 MB of wf per buffer (1 GB of scratch per encoder stream out of 180 GB); larger layers are cut into
+// stage 1 of chunk i+1). Every chunk costs a stage-1 tail, a GEMM launch with its fixed latency and a partial wave,
+// and both kernels fill the machine on their own so the overlap buys little, while HBM takes the wf round trip of the
+// largest layer in well under the stage-1 time. So: one chunk per layer up to 512 MB of wf per buffer (1 GB of scratch
+// per encoder stream out of the 80 GB of an H100); larger layers are cut into
 // equal chunks of that size.
 static int chunk_queries(int K, int Cin) {
   static const int forced = [] { const char* v = getenv("D3F_KPCONV_CHUNK"); return v ? atoi(v) : 0; }();

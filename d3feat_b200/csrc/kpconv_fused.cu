@@ -9,22 +9,16 @@
 //                               wf[16 kp x 32 ch] += w^T . f on the tensor pipe (mma.sync m16n8k8, 3xTF32), x 1/nn, then
 //                               the query's wf row is split (hi, lo) and written STRAIGHT into the shared-memory operand
 //                               of the contraction: per kernel point [48 hi rows | 48 lo rows] x 128 B, K-major
-//                               SWIZZLE_128B, the layout the UMMA descriptors read.
-//   control warp 15 (lane 0)    W ring producer (TMA bulk copies of pre-swizzled 8 KB images, 4 stages) and MMA issuer:
-//                               out^T[64 x 96] += Wimg[kp] (64 rows = TF32-hi and remainder of the 32 output channels) .
-//                               [wf_hi | wf_lo][:, kp, :]^T on tcgen05 (kind::tf32, M = 64, N = 96, ONE MMA per K = 8
-//                               step, 60 per tile), accumulators in TMEM (two, alternating MMA by MMA; double-buffered
-//                               across tiles so that the epilogue of tile k runs under the MMAs of tile k + 1).
-//   epilogue warps 16..19       one TMEM lane quadrant each: tcgen05.ld -> hi + lo rows, hi + lo columns ->
+//                               SWIZZLE_128B, the layout the wgmma descriptors read.
+//   control warp 15 (lane 0)    W ring producer: TMA bulk copies of pre-swizzled 8 KB images, 4 stages.
+//   MMA warpgroup 16..19        out^T[64 x 96] += Wimg[kp] (64 rows = TF32-hi and remainder of the 32 output channels) .
+//                               [wf_hi | wf_lo][:, kp, :]^T on wgmma (tf32, M = 64, N = 96, ONE wgmma per K = 8 step,
+//                               60 per tile), accumulator in registers; then hi + lo rows, hi + lo columns ->
 //                               batch-norm affine -> bias -> LeakyReLU -> out.
 //
 // Tile shape: the wf operand of a tile is 15 kernel points x [48 hi rows | 48 lo rows] x 128 B = 180 KB and shares the
 // 227 KB of an SM with a 4-stage ring of 8 KB W images. One tile in flight: the gather warps are already inside their
 // next queries while its 60 MMAs run; only the WRITE of the next tile's rows waits for them (`consumed` counter).
-// What was tried on the way (all measured, profiles/r2_notes.md): queries on M (three M = 128 MMAs per K step, 15 KB of
-// operand reads each step), a 40-row tile with an 8-stage ring, two 24-row tiles (double-buffered; the per-tile cost of
-// 120 small MMAs and of re-streaming W every 24 queries made the contraction the bottleneck), an issuer that also
-// refilled the W ring / ran a quadrant's epilogue (each serialised the MMA issue).
 #include <stdlib.h>
 
 #include "ops.cuh"
@@ -36,8 +30,8 @@ namespace {
 
 constexpr int kFRows = 48;                       // queries per tile (see "Tile shape" above)
 constexpr int kFGatherWarps = 15;                // rows are handed out dynamically
-constexpr int kFCtrlWarp = 15;                   // lane 0: W ring producer + MMA issuer, nothing else
-constexpr int kFEpiWarp0 = 16;                   // warps 16..19: epilogue of TMEM lane quadrant (warp % 4)
+constexpr int kFCtrlWarp = 15;                   // lane 0: W ring producer, nothing else
+constexpr int kFEpiWarp0 = 16;                   // warps 16..19: the MMA warpgroup (wgmma + epilogue)
 constexpr int kFThreads = 20 * 32;
 // (20 warps = 5 per SM sub-partition: 5 x 32 x 96 registers fit its 16 K registers; a 21st warp would cap everyone at 80)
 constexpr int kFKp = 15;
@@ -52,8 +46,8 @@ struct FusedSmem {
   static constexpr int kWBytes = kFWStages * kFWStage;
   static constexpr int kBarOff = kFABytes + kWBytes;                  // mbarriers
   static constexpr int kNumBars = 8 + 2 * kFWStages;
-  static constexpr int kTmemSlotOff = kBarOff + kNumBars * 8;        // then the row counter and the consumed counter
-  static constexpr int kTotal = kTmemSlotOff + 16 + 1024 /*alignment slack*/;
+  static constexpr int kCtrOff = kBarOff + kNumBars * 8;             // the row counter and the consumed counter
+  static constexpr int kTotal = kCtrOff + 16 + 1024 /*alignment slack*/;
   static_assert(kTotal <= 232448, "shared memory budget of an SM (227 KB)");
 };
 
@@ -107,20 +101,6 @@ __device__ __forceinline__ void mbar_wait_sleep(uint32_t bar, uint32_t parity) {
   }
 }
 
-// NON-blocking test (mbarrier.test_wait): try_wait may suspend the thread for a system-dependent time before it returns
-// false, which stalled the control thread's polling loops for microseconds at a time (2.7 ms instead of 0.7 ms)
-__device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-
 // position of a gather warp in its stream of (tile, query slot, 8-neighbour step)
 // (rows are handed out dynamically: rowg = k * 48 + row counts the rows of this CTA's tile sequence)
 struct Pos {
@@ -137,40 +117,6 @@ struct StepData {
 
 }  // namespace
 
-// tcgen05.ld of N consecutive 32-bit columns of this warp's 32 TMEM lanes
-template <int N>
-__device__ __forceinline__ void tmem_ld(uint32_t taddr, float* v);
-template <>
-__device__ __forceinline__ void tmem_ld<32>(uint32_t taddr, float* v) {
-  float t[32];
-  tmem_ld32(taddr, *reinterpret_cast<float(*)[32]>(t));
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = t[i];
-}
-template <>
-__device__ __forceinline__ void tmem_ld<16>(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                 "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-               : "r"(taddr)
-               : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-template <>
-__device__ __forceinline__ void tmem_ld<8>(uint32_t taddr, float* v) {
-  uint32_t r[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-
 __global__ void __launch_bounds__(kFThreads, 1) kpconv_fused32_kernel(FusedParams pin) {
   FusedParams p = pin;
   p.Nq = dyn_rows(pin.Nq, pin.nq_dev);
@@ -181,17 +127,14 @@ __global__ void __launch_bounds__(kFThreads, 1) kpconv_fused32_kernel(FusedParam
   uint8_t* smem = (uint8_t*)(((uintptr_t)fused_smem_raw + 1023) & ~(uintptr_t)1023);
   const uint32_t sbase = smem_u32(smem);
   uint64_t* bars = (uint64_t*)(smem + S_::kBarOff);
-  // bars: 0 a_full (all lanes of the warps that wrote the tile's rows), 3,4 acc_done[TMEM half] (MMA commit),
-  //       5,6 epi_done[TMEM half] (the four epilogue warps), 8.. w_full[kWS], then w_empty[kWS]
+  // bars: 0 a_full (all lanes of the warps that wrote the tile's rows), 8.. w_full[kWS], then w_empty[kWS]
   const uint32_t bar_a_full = smem_u32(&bars[0]);
-  const uint32_t bar_acc0 = smem_u32(&bars[3]), bar_epi0 = smem_u32(&bars[5]);
   constexpr int kWB = 8;   // first W barrier
-  uint32_t* tmem_slot = (uint32_t*)(smem + S_::kTmemSlotOff);
-  int* row_ctr = (int*)(smem + S_::kTmemSlotOff + 8);   // next row of this CTA's tile sequence (gather warps)
+  int* row_ctr = (int*)(smem + S_::kCtrOff);       // next row of this CTA's tile sequence (gather warps)
   // number of this CTA's tiles whose MMAs have retired. A plain counter, not an mbarrier: a gather warp may skip several
   // tiles (its rows are taken by the others), and a parity wait on a barrier that is two or more phases ahead waits for
   // a FUTURE phase -- with the warp's own row part of that future tile, a deadlock.
-  int* consumed = (int*)(smem + S_::kTmemSlotOff + 12);
+  int* consumed = (int*)(smem + S_::kCtrOff + 4);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int tiles = ceil_div(p.Nq, kFRows);
@@ -203,26 +146,13 @@ __global__ void __launch_bounds__(kFThreads, 1) kpconv_fused32_kernel(FusedParam
     *row_ctr = 0;
     *consumed = 0;
     mbar_init(bar_a_full, kFRows * 32);              // every lane of the warp that produced a row arrives for it
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(bar_acc0 + 8 * b, 1);
-      mbar_init(bar_epi0 + 8 * b, 4);
-    }
     for (int s = 0; s < kWS; ++s) {
       mbar_init(smem_u32(&bars[kWB + s]), 1);
-      mbar_init(smem_u32(&bars[kWB + kWS + s]), 1);
+      mbar_init(smem_u32(&bars[kWB + kWS + s]), 4);  // one arrive per warp of the MMA warpgroup
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == kFEpiWarp0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(512u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < kFGatherWarps) {
     // =========================== gather / stage-1 warps ==================================================
@@ -236,8 +166,8 @@ __global__ void __launch_bounds__(kFThreads, 1) kpconv_fused32_kernel(FusedParam
     const float* fcol = p.feat + 4 * g;      // lane (g, t): channels [4g, 4g+4) of its neighbours' rows
 
     // Rows are handed out one at a time from a shared counter: a warp takes its next row two steps before it finishes
-    // the current one. A static split (3 rows per warp and tile) made every warp wait for the slowest one at every
-    // tile (32 % of the stall samples sat in the a_free wait, profiles/r2_notes.md).
+    // the current one: with a static split (3 rows per warp and tile) every warp would wait for the slowest one at
+    // every tile.
     const int total_rows = my_tiles * kFRows;
     int static_next = warp;
     auto grab = [&]() {
@@ -418,112 +348,75 @@ __global__ void __launch_bounds__(kFThreads, 1) kpconv_fused32_kernel(FusedParam
       step(dB, dA, iA, iB);
     }
   } else if (warp == kFCtrlWarp) {
-    // =========================== control thread: W ring producer + MMA issuer ======================================
-    // Swapped orientation: D^T[64 x 96] = Wimg[64 x 32ch] . [wf_hi(48 rows) | wf_lo(48 rows)]^T per kernel point and
-    // K = 8 step. The 64 rows of a W image are the 32 output channels twice (TF32-hi and the exact remainder, 8 + 8 per
-    // TMEM lane quadrant), the 96 operand rows are the tile's queries twice (hi and lo of their wf), so ONE MMA yields
-    // Wh.wf_hi, Wl.wf_hi, Wh.wf_lo (and the negligible Wl.wf_lo): 60 MMAs per 48 queries. (Measured on the way here,
-    // profiles/r2_notes.md: with queries on M the contraction read 15 KB of operands per K step against 128 B/clk; a
-    // TF32 MMA of this size costs ~55-100 cycles whatever N is, so the instruction count per query is what matters.)
-    // The thread does nothing else: an issuer that also refilled the ring or ran an epilogue was the bottleneck twice.
+    // =========================== control thread: W ring producer ===================================================
+    // The W image of every kernel point of every tile, in the order the MMA warpgroup consumes them.
     if (lane == 0) {
-      const uint32_t idesc = make_idesc_tf32(64, 2 * kFRows);
       const int total_chunks = my_tiles * kFKp;
-      int pc = 0;                                       // next W chunk to load
-      auto produce = [&]() {
-        while (pc < total_chunks) {
-          const int st = pc % kWS;
-          if (pc >= kWS && !mbar_try(smem_u32(&bars[kWB + kWS + st]), (uint32_t)((pc / kWS - 1) & 1))) return;
-          const uint32_t full = smem_u32(&bars[kWB + st]);
-          mbar_arrive_expect_tx(full, (uint32_t)kFWStage);
-          tma_bulk_g2s(sbase + kFABytes + (uint32_t)st * kFWStage, p.Wp + (size_t)(pc % kFKp) * (kFWStage / 4),
-                       (uint32_t)kFWStage, full);
-          ++pc;
-        }
-      };
-      auto wait_producing = [&](uint32_t bar, uint32_t parity, unsigned ns) {
-        while (!mbar_try(bar, parity)) {
-          produce();
-          if (ns) __nanosleep(ns);
-        }
-      };
-      produce();
-      int it = 0;
-      for (int tile = blockIdx.x; tile < tiles; tile += tstride, ++it) {
-        const uint32_t h = (uint32_t)(it & 1);
-        wait_producing(bar_a_full, (uint32_t)(it & 1), 64);          // all 48 rows of the tile are in shared memory
-        if (it >= 2) wait_producing(bar_epi0 + 8 * h, (uint32_t)(((it - 2) >> 1) & 1), 32);   // TMEM half h was read
-        tc_fence_after();
-        for (int kp = 0; kp < kFKp; ++kp) {
-          const int c = it * kFKp + kp;
-          const int st = c % kWS;
-          wait_producing(smem_u32(&bars[kWB + st]), (uint32_t)((c / kWS) & 1), 0);
-          tc_fence_after();
-          const uint64_t dw = make_smem_desc(sbase + kFABytes + (uint32_t)st * kFWStage);
-          const uint64_t df = make_smem_desc(sbase + (uint32_t)kp * kFChunkBytes);
-          // two accumulators (128 TMEM columns apart), alternating MMA by MMA
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint64_t adv = (uint64_t)((j * 32) >> 4);   // +32 B per K = 8 step inside the swizzle atom
-            umma_tf32(tmem_base + 256u * h + (uint32_t)((j & 1) * 128), dw + adv, df + adv, idesc,
-                      (kp == 0 && j < 2) ? 0u : 1u);
-          }
-          umma_commit(smem_u32(&bars[kWB + kWS + st]));          // W stage free once these MMAs retire
-          produce();
-        }
-        umma_commit(bar_acc0 + 8 * h);       // accumulators of this half complete (and the wf tile is free)
+      for (int pc = 0; pc < total_chunks; ++pc) {
+        const int st = pc % kWS;
+        if (pc >= kWS) mbar_wait_sleep(smem_u32(&bars[kWB + kWS + st]), (uint32_t)((pc / kWS - 1) & 1));
+        const uint32_t full = smem_u32(&bars[kWB + st]);
+        mbar_arrive_expect_tx(full, (uint32_t)kFWStage);
+        tma_bulk_g2s(sbase + kFABytes + (uint32_t)st * kFWStage, p.Wp + (size_t)(pc % kFKp) * (kFWStage / 4),
+                     (uint32_t)kFWStage, full);
       }
     }
   } else {
-    // =========================== epilogue warps: one TMEM lane quadrant each =======================================
-    // With M = 64 the accumulator rows 16 qd .. 16 qd + 15 live in TMEM lanes 32 qd .. 32 qd + 15: lanes 0-7 of warp qd
-    // hold the Wh rows of output channels 8 qd .. 8 qd + 7, lanes 8-15 their Wl rows; columns 0-47 are the queries against
-    // wf_hi, 48-95 against wf_lo. out[n, c] = (acc0 + acc1)(hi row + lo row)(col j + col 48 + j).
+    // =========================== MMA warpgroup (warps 16..19): contraction + epilogue ==============================
+    // Swapped orientation: D^T[64 x 96] = Wimg[64 x 32ch] . [wf_hi(48 rows) | wf_lo(48 rows)]^T per kernel point and
+    // K = 8 step. The 64 rows of a W image are the 32 output channels twice (TF32-hi and the exact remainder, 8 + 8 per
+    // 16-row slab of a warp), the 96 operand rows are the tile's queries twice (hi and lo of their wf), so ONE wgmma
+    // yields Wh.wf_hi, Wl.wf_hi, Wh.wf_lo (and the negligible Wl.wf_lo): 60 wgmmas per 48 queries. The gather warps are
+    // already writing the next tile's rows while this warpgroup runs the epilogue.
     const int qd = warp - kFEpiWarp0;
-    const int co = 8 * qd + (lane & 7);
+    // accumulator fragment (tc_common.cuh): rows 16 qd + lane / 4 (Wh of channel co) and + 8 (Wl of channel co),
+    // columns 8 j + 2 (lane % 4) + e: query 8 j + 2 (lane % 4) + e against wf_hi for j < 6, against wf_lo for j >= 6
+    const int co = 8 * qd + (lane >> 2);
     const float e_sc = p.bn_scale ? p.bn_scale[co] : 1.f, e_sh = p.bn_scale ? p.bn_shift[co] : 0.f;
     const float e_bi = p.bias ? p.bias[co] : 0.f;
+    float acc[48];
     int it = 0;
     for (int tile = blockIdx.x; tile < tiles; tile += tstride, ++it) {
-      const uint32_t h = (uint32_t)(it & 1);
-      mbar_wait_sleep(bar_acc0 + 8 * h, (uint32_t)((it >> 1) & 1));
-      tc_fence_after();
-      if (qd == 1 && lane == 0)   // the MMAs of tile it have retired: the wf tile may be overwritten
+      mbar_wait_sleep(bar_a_full, (uint32_t)(it & 1));          // all 48 rows of the tile are in shared memory
+#pragma unroll
+      for (int j = 0; j < 48; ++j) acc[j] = 0.f;
+      for (int kp = 0; kp < kFKp; ++kp) {
+        const int c = it * kFKp + kp;
+        const int st = c % kWS;
+        mbar_wait(smem_u32(&bars[kWB + st]), (uint32_t)((c / kWS) & 1));
+        wgmma_fence();
+        const uint64_t dw = make_smem_desc(sbase + kFABytes + (uint32_t)st * kFWStage);
+        const uint64_t df = make_smem_desc(sbase + (uint32_t)kp * kFChunkBytes);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const uint64_t adv = (uint64_t)((j * 32) >> 4);   // +32 B per K = 8 step inside the swizzle atom
+          wgmma_tf32<96>(acc, dw + adv, df + adv);
+        }
+        wgmma_commit();
+        if (kp > 0) {                                          // the previous kernel point's W stage is free
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(smem_u32(&bars[kWB + kWS + (c - 1) % kWS]));
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_reg_fence<48>(acc);
+      if (lane == 0) mbar_arrive(smem_u32(&bars[kWB + kWS + (it * kFKp + kFKp - 1) % kWS]));
+      asm volatile("bar.sync 1, 128;" ::: "memory");          // every warp's wgmmas of this tile have retired
+      if (qd == 0 && lane == 0)   // the wf tile may be overwritten
         asm volatile("st.release.cta.shared.b32 [%0], %1;" ::"r"(smem_u32(consumed)), "r"(it + 1) : "memory");
-      const uint32_t t0 = tmem_base + ((uint32_t)(32 * qd) << 16) + 256u * h;
-#pragma unroll 1
-      for (int cb = 0; cb < kFRows; cb += 16) {
-        float v[16], w2[16];
-        tmem_ld<16>(t0 + (uint32_t)cb, v);
-        tmem_ld<16>(t0 + (uint32_t)(kFRows + cb), w2);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] += w2[j];
-        tmem_ld<16>(t0 + 128u + (uint32_t)cb, w2);
+      for (int j = 0; j < 6; ++j) {
 #pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] += w2[j];
-        tmem_ld<16>(t0 + 128u + (uint32_t)(kFRows + cb), w2);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          float x = v[j] + w2[j];
-          x += __shfl_down_sync(0xffffffffu, x, 8);      // hi row (lane) + lo row (lane + 8)
-          const int n = tile * kFRows + cb + j;
-          if (lane < 8 && n < p.Nq) {
+        for (int e = 0; e < 2; ++e) {
+          float x = (acc[4 * j + e] + acc[4 * j + 2 + e]) + (acc[4 * (j + 6) + e] + acc[4 * (j + 6) + 2 + e]);
+          const int n = tile * kFRows + 8 * j + 2 * (lane & 3) + e;
+          if (n < p.Nq) {
             x = fmaf(x, e_sc, e_sh) + e_bi;
             if (p.leaky_alpha >= 0.f) x = x > 0.f ? x : x * p.leaky_alpha;
             p.out[(size_t)n * 32 + co] = x;
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_epi0 + 8 * h);
-    }
-    if (qd == 0) {
-      // every warp's TMEM reads are done once the last two tiles' epilogues have been signalled by all four warps
-      if (it >= 1) mbar_wait(bar_epi0 + 8 * (uint32_t)((it - 1) & 1), (uint32_t)(((it - 1) >> 1) & 1));
-      if (it >= 2) mbar_wait(bar_epi0 + 8 * (uint32_t)((it - 2) & 1), (uint32_t)(((it - 2) >> 1) & 1));
-      tc_fence_after();
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
     }
   }
 }
@@ -531,7 +424,7 @@ __global__ void __launch_bounds__(kFThreads, 1) kpconv_fused32_kernel(FusedParam
 // W[15][32][32] (K_values of a 32 -> 32 KPConv) -> 15 shared-memory images of [64 rows][32 channels]: row r of quadrant
 // qd = r / 16 holds output channel 8 qd + (r % 8), rows with (r % 16) < 8 its TF32-rounded value, the others the exact
 // remainder; K-major SWIZZLE_128B (16-byte chunks XOR-ed with r % 8), i.e. ready to be dropped into an SM by one TMA
-// bulk copy and read by the UMMA descriptor.
+// bulk copy and read by the wgmma descriptor.
 __global__ void __launch_bounds__(256) pack_weight_fused32_kernel(const float* __restrict__ W, float* __restrict__ img) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= kFKp * 64 * 32) return;
@@ -548,10 +441,8 @@ __global__ void __launch_bounds__(256) pack_weight_fused32_kernel(const float* _
 // aggregation, Cout = 32, 16-byte aligned features, and enough queries to fill the GPU.
 bool kpconv_fused_supported(int Nq, int H, int K, int Cin, int Cout, int influence, int mode, const float* feat,
                             const float* W, const float* out, const int* query_order) {
-  // D3F_FUSED_KPCONV=1 selects this kernel. Default off: measured on B200 (profiles/r2_notes.md) it equals the
-  // two-kernel path in isolation (0.75 vs 0.72 ms at 240k queries, with 5x less DRAM traffic) but costs the pipelined
-  // step 0.2 ms, because a persistent 227 KB-per-SM CTA leaves no room for the pyramid kernels of the next batch that
-  // the two-stream pipeline overlaps with the encoder.
+  // D3F_FUSED_KPCONV=1 selects this kernel. Default off: a persistent 227 KB-per-SM CTA leaves no room for the
+  // pyramid kernels of the next batch that the two-stream pipeline overlaps with the encoder.
   const char* v = getenv("D3F_FUSED_KPCONV");
   if (v == nullptr || v[0] != '1') return false;
   return H >= 1 && K == kFKp && Cin == 32 && Cout == 32 && influence == D3F_INFLUENCE_LINEAR &&

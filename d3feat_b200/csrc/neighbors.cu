@@ -417,9 +417,8 @@ radius_query_kernel(const float* __restrict__ q, int Nq_cap, const int* __restri
 }
 
 // ---------------------------------------------------------------------------------------------------
-// The same query with TWO queries per warp (16 lanes each). ncu of the kernel above (profiles/r2_radius_query_ncu.txt):
-// instruction bound, ~600 warp instructions per query of which 165 are the prologue (nine lanes busy) and ~170 the
-// 64-key sort (two keys per lane, 15 of 21 exchange levels through shuffles). With 16 lanes per query the prologue
+// The same query with TWO queries per warp (16 lanes each). The kernel above is instruction bound: a large share of a
+// query's warp instructions is the prologue (nine lanes busy) and the 64-key sort (two keys per lane, 15 of 21 exchange levels through shuffles). With 16 lanes per query the prologue
 // serves two queries per warp instruction and a lane holds FOUR keys (elements 4 l .. 4 l + 3): only the exchanges at
 // distance >= 4 need a shuffle (10 of 21 levels). The candidate loop is unchanged in lane efficiency (~110 candidates
 // in steps of 16; the warp runs to the longer of its two lists).

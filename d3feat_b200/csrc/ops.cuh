@@ -18,7 +18,7 @@ struct Epilogue {
 };
 int gemm_f32(const float* A, const float* B, float* C, int M, int N, int K, const Epilogue& ep, cudaStream_t stream);
 
-// ---- tc_gemm.cu (tcgen05 / TMEM, 3xTF32) ------------------------------------------------------------
+// ---- tc_gemm.cu (wgmma, 3xTF32) ---------------------------------------------------------------------
 size_t tc_packed_floats(int K, int N);
 int tc_padded_n(int N);
 int tc_pack_weight(const float* W, int K, int N, float* packed, cudaStream_t stream);
@@ -72,7 +72,7 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
                         float* out, void* workspace, size_t workspace_bytes, cudaStream_t stream,
                         const int* nq_dev = nullptr, const int* ns_dev = nullptr);
 
-// ---- kpconv_fused.cu (one persistent kernel per layer: gather + correlation + tcgen05 contraction) -----
+// ---- kpconv_fused.cu (one persistent kernel per layer: gather + correlation + wgmma contraction) -------
 bool kpconv_fused_supported(int Nq, int H, int K, int Cin, int Cout, int influence, int mode, const float* feat,
                             const float* W, const float* out, const int* query_order);
 size_t kpconv_fused_workspace_bytes();

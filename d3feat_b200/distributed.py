@@ -1,5 +1,5 @@
 """Multi-GPU: whole point-cloud fragments shard across ranks (one process per GPU); the only exchange step is
-ONE all-gather of the per-fragment descriptors at the end (NCCL over NVLink/NVSwitch on the B200 box, gloo in
+ONE all-gather of the per-fragment descriptors at the end (NCCL over NVLink/NVSwitch between H100s, gloo in
 the CPU tests). The reference is single-process (SURVEY.md 8e): fragments are independent units, so there is no
 data-path collective inside the pyramid or the encoder.
 """

@@ -190,8 +190,8 @@ class GraphPipeline:
         pipe.drain(); pipe.check()                                 # status bits: capacity overflow / points out of bounds
 
     `res` is the slot's static output buffer [capacity of the last level, C] and `counts` the device int32 level sizes
-    (rows beyond counts[-1] are undefined); both stay valid until the slot is reused DEPTH steps later. Mirrors the
-    overlap the reference gets from tf.data prefetch (datasets/common.py:744-763)."""
+    (counts[l] for level l < L; rows of `res` beyond counts[L - 1] are undefined); both stay valid until the slot is
+    reused DEPTH steps later. Mirrors the overlap the reference gets from tf.data prefetch (datasets/common.py:744-763)."""
 
     DEPTH = 4
 
@@ -203,7 +203,7 @@ class GraphPipeline:
         self.bbox = np.ascontiguousarray(bbox, np.float32)
         self.s_pyr = torch.cuda.Stream(device=dev)
         # Encoders of consecutive batches alternate between `encoder_streams` streams: the deep pyramid levels (a few
-        # thousand rows) cannot fill 148 SMs on their own, so the tail of encoder(i) runs under the level-0 kernels of
+        # thousand rows) cannot fill 132 SMs on their own, so the tail of encoder(i) runs under the level-0 kernels of
         # encoder(i + 1). Results still come back in batch order (each step waits for its own batch's event).
         self.s_encs = [torch.cuda.Stream(device=dev) for _ in range(max(1, int(encoder_streams)))]
         self.s_enc = self.s_encs[0]

@@ -232,7 +232,6 @@ def descriptor_input(config, stacked_points, stacked_lengths, neighborhood_limit
             out["upsamples"].append(empty_i)
         out["orders"].append(torch.zeros((0,), dtype=i32, device=dev))
     # D3F_QUERY_ORDER=1: hand the level-0 gather kernels the hash grid's cell order as query visiting order
-    # (measured on B200: no gain -- the gathers are L2-latency bound, not locality bound; profiles/r1_notes.md)
     if os.environ.get("D3F_QUERY_ORDER", "0") == "1" and levels[0]["conv_r"] is not None:
         out["orders"][0] = ops.NeighborGrid(pts, lens, levels[0]["conv_r"], bb).order()
     return out

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's native ops (tf_custom_ops/), backed by the sm_100a hash-grid kernels.
+"""Host-side mirror of the reference's native ops (tf_custom_ops/), backed by the sm_90a hash-grid kernels.
 
 Reference interface                                   -> here
   tf_batch_neighbors_module.batch_ordered_neighbors   -> batch_ordered_neighbors   (tf_batch_neighbors.cpp:8-30)

@@ -1,4 +1,4 @@
-/* d3feat_b200 -- C ABI of the Blackwell-native (sm_100a) D3Feat hot path.
+/* d3feat_b200 -- C ABI of the Hopper-native (sm_90a) D3Feat hot path.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch / TF types. Every entry point
  *   - takes DEVICE pointers unless a parameter is explicitly marked "host",
@@ -161,10 +161,10 @@ int d3f_pyramid_build(const float* points, const int* lengths, int B, int N0,
 
 /* ---------------------------------------------------------------------------------------------
  * Static weights for the tensor-core path. A weight matrix W[K,N] (row-major; for KPConv the [K*Cin, Cout]
- * view of K_values[K,Cin,Cout]) is packed ONCE into the K-major TF32 hi/lo images the tcgen05 kernels
+ * view of K_values[K,Cin,Cout]) is packed ONCE into the K-major TF32 hi/lo images the wgmma kernels
  * consume (3xTF32 split: fp32-level accuracy on the 5th-gen tensor cores). Every forward entry point takes
  * the packed image as an optional `W_packed` argument: NULL selects the CUDA-core fp32 path (same results
- * within rounding), non-NULL the tcgen05 path.
+ * within rounding), non-NULL the wgmma path.
  * ------------------------------------------------------------------------------------------- */
 size_t d3f_packed_weight_floats(int K, int N);
 int d3f_pack_weight(const float* W, int K, int N, float* packed, d3f_stream_t stream);

@@ -1,4 +1,4 @@
-"""GPU: time the tcgen05 GEMM at the encoder's characteristic shapes (CUDA events, warm)."""
+"""GPU: time the wgmma GEMM at the encoder's characteristic shapes (CUDA events, warm)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

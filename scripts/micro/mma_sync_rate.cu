@@ -1,4 +1,5 @@
-// Microbenchmark: throughput of legacy mma.sync.m16n8k8 (tf32) on sm_100a, per SM and whole chip.
+// Microbenchmark: throughput of legacy mma.sync.m16n8k8 (tf32) on sm_90a, per SM and whole chip.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 mma_sync_rate.cu -o mma_sync_rate
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void k(float* out, int iters) {
@@ -17,17 +18,24 @@ __global__ void k(float* out, int iters) {
   out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 int main() {
-  float* d; cudaMalloc(&d, 148 * 8 * 512 * 4);
+  cudaDeviceProp prop;
+  cudaGetDeviceProperties(&prop, 0);
+  const int sms = prop.multiProcessorCount;
+  int khz = 0;
+  cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
+  const double hz = khz * 1e3;   // maximum SM clock: the per-clock figures assume the card holds it
+  float* d; cudaMalloc(&d, (size_t)sms * 2 * 16 * 32 * 4);
   for (int warps = 4; warps <= 16; warps *= 2) {
     int iters = 20000;
-    k<<<148 * 2, warps * 32>>>(d, 10); cudaDeviceSynchronize();
+    k<<<sms * 2, warps * 32>>>(d, 10); cudaDeviceSynchronize();
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    cudaEventRecord(e0); k<<<148 * 2, warps * 32>>>(d, iters); cudaEventRecord(e1); cudaEventSynchronize(e1);
+    cudaEventRecord(e0); k<<<sms * 2, warps * 32>>>(d, iters); cudaEventRecord(e1); cudaEventSynchronize(e1);
     float ms; cudaEventElapsedTime(&ms, e0, e1);
-    double mmas = 148.0 * 2 * warps * iters * 4;
+    double mmas = (double)sms * 2 * warps * iters * 4;
     double flops = mmas * 16 * 8 * 8 * 2;
-    printf("warps/CTA=%2d (2 CTAs/SM): %.3f ms, %.1f TFLOP/s tf32, %.2f MMA/clk/SM @1.9GHz, cycles per MMA per SMSP = %.1f\n", warps, ms,
-           flops / ms / 1e9, mmas / (ms * 1e-3) / 148 / 1.9e9, 4.0 / (mmas / (ms * 1e-3) / 148 / 1.9e9));
+    const double per_clk = mmas / (ms * 1e-3) / sms / hz;
+    printf("warps/CTA=%2d (2 CTAs/SM): %.3f ms, %.1f TFLOP/s tf32, %.2f MMA/clk/SM @%.2f GHz, cycles per MMA per SMSP = %.1f\n",
+           warps, ms, flops / ms / 1e9, per_clk, hz / 1e9, 4.0 / per_clk);
   }
   printf("%s\n", cudaGetErrorString(cudaGetLastError()));
   return 0;

@@ -3,7 +3,7 @@
     python scripts/run_released_model.py --log /path/to/results/Log_contraloss --out out_dir a.ply b.ply ...
 
 (the demo_registration.py / tester.generate_descriptor flow: voxelise at first_subsampling_dl, features = ones,
-model -> [N,32] descriptors and [N,1] scores, rows written in ascending score order). Needs a B200.
+model -> [N,32] descriptors and [N,1] scores, rows written in ascending score order). Needs an H100 (sm_90a).
 """
 import argparse
 import glob

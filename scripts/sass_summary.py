@@ -1,6 +1,6 @@
 """CPU box: per-kernel SASS evidence of what each kernel is built from (cuobjdump of the objects in d3feat_b200/build):
-tcgen05.mma (UTC*MMA), tcgen05.ld (LDTM), TMA (UBLKCP / UTMALDG), legacy mma.sync (HMMA), cp.async (LDGSTS), mbarrier
-(SYNCS), registers. Writes profiles/sass_summary.txt."""
+wgmma (HGMMA), TMA (UBLKCP / UTMALDG), legacy mma.sync (HMMA), cp.async (LDGSTS), mbarrier (SYNCS), registers.
+Writes profiles/sass_summary.txt."""
 import glob
 import os
 import re
@@ -8,9 +8,9 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-pat = ["UTCHMMA", "UTCQMMA", "LDTM", "UBLKCP", "UTMALDG", "HMMA", "LDGSTS", "SYNCS", "ATOMG", "RED", "MUFU", "LDG", "STG", "LDS", "STS"]
-out = ["# SASS mnemonic counts per kernel (cuobjdump -sass of d3feat_b200/build/*.o, sm_100a)",
-       "# tcgen05.mma -> UTC*MMA, tcgen05.ld -> LDTM, cp.async.bulk (TMA) -> UBLKCP / UTMALDG, mma.sync -> HMMA, cp.async -> LDGSTS",
+pat = ["HGMMA", "UBLKCP", "UTMALDG", "HMMA", "LDGSTS", "SYNCS", "ATOMG", "RED", "MUFU", "LDG", "STG", "LDS", "STS"]
+out = ["# SASS mnemonic counts per kernel (cuobjdump -sass of d3feat_b200/build/*.o, sm_90a)",
+       "# wgmma.mma_async -> HGMMA, cp.async.bulk (TMA) -> UBLKCP / UTMALDG, mma.sync -> HMMA, cp.async -> LDGSTS",
        "%-64s %5s " % ("kernel", "regs") + " ".join("%7s" % p for p in pat)]
 for obj in sorted(glob.glob(os.path.join(ROOT, "d3feat_b200", "build", "*.o"))):
     sass = subprocess.run(["cuobjdump", "-sass", obj], capture_output=True, text=True).stdout
@@ -36,5 +36,6 @@ for obj in sorted(glob.glob(os.path.join(ROOT, "d3feat_b200", "build", "*.o"))):
         dem = subprocess.run(["cu++filt", fn], capture_output=True, text=True).stdout.strip() or fn
         dem = re.sub(r"\(.*", "", dem.replace("(int)", "").replace("(bool)", "")).replace("void ", "").replace("d3f::", "").replace("(anonymous namespace)::", "")
         out.append("%-64s %5s " % (dem[:64], regs.get(fn, "?")) + " ".join("%7d" % c[p] for p in pat))
+os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
 open(os.path.join(ROOT, "profiles", "sass_summary.txt"), "w").write("\n".join(out) + "\n")
-print("\n".join(l for l in out if "UTC" in l or "fused" in l or "tc_gemm" in l or l.startswith("#"))[:3000])
+print("\n".join(l for l in out if "HGMMA" in l or "fused" in l or "tc_gemm" in l or l.startswith("#"))[:3000])

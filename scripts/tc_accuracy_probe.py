@@ -1,4 +1,4 @@
-"""GPU probe: max-norm relative error of the tcgen05 3xTF32 GEMM vs float64 as a function of K."""
+"""GPU probe: max-norm relative error of the wgmma 3xTF32 GEMM vs float64 as a function of K."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

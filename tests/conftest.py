@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on a machine with an H100)")
 
 
 @pytest.fixture(scope="session")
@@ -20,6 +20,16 @@ def golden():
 
     def load(name):
         return np.load(os.path.join(GOLDEN, name))
+    return load
+
+
+@pytest.fixture(scope="session")
+def golden_json():
+    import json
+
+    def load(name):
+        with open(os.path.join(GOLDEN, name)) as fh:
+            return json.load(fh)
     return load
 
 

@@ -1,12 +1,11 @@
 """Formats either side of the hot path (SURVEY.md §8 f3/f4): TF checkpoint bundles, parameters.txt, PLY, and the
 per-fragment output arrays. CPU only.
 
-Known answers from the reference's own artefacts (read only where /root/reference exists, i.e. in the build
-container): the 10 kernel-point tensors inside results_kitti/Log_11011605/snapshots/snap-61 must equal the
-kernel_points/epoch61/*.ply files the trainer wrote from the same variables, bit for bit, and the variable names
-of all three released snapshots must be exactly the names the host mirror looks up.
+Known answers from the reference's released artefacts (tests/golden/released_checkpoints.npz, written by
+scripts/make_released_golden.py): the 10 kernel-point tensors inside results_kitti/Log_11011605/snapshots/snap-61 must
+equal the kernel_points/epoch61/*.ply files the trainer wrote from the same variables, bit for bit, and the variable
+names of all three released snapshots must be exactly the names the host mirror looks up.
 """
-import glob
 import os
 
 import numpy as np
@@ -15,8 +14,30 @@ import pytest
 from d3feat_b200 import io_utils, synth
 from d3feat_b200 import tf_checkpoint as ck
 
-REF = "/root/reference"
-needs_ref = pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not present on this machine")
+RELEASED = (("kitti61", 61), ("contraloss54", 54), ("circleloss48", 48))
+
+
+@pytest.fixture(scope="module")
+def released(golden):
+    z = golden("released_checkpoints.npz")
+    return {k: z[k] for k in z.files}
+
+
+def released_snapshot(released, tag, snap, where, payloads=()):
+    """The released snapshot's real index next to a sparse data file of the real size that holds only the payloads
+    the fixture keeps (at their real offsets): read_checkpoint verifies them against the CRC32C of the real index."""
+    prefix = os.path.join(str(where), tag, "snap-%d" % snap)
+    os.makedirs(os.path.dirname(prefix))
+    released[tag + "|index"].tofile(prefix + ".index")
+    _, entries = ck.read_index(prefix)
+    with open(prefix + ".data-00000-of-00001", "wb") as fh:
+        fh.truncate(int(released[tag + "|data_size"]))
+        for name in payloads:
+            fh.seek(entries[name]["offset"])
+            fh.write(released[tag + "|data|" + name].tobytes())
+    with open(os.path.join(os.path.dirname(prefix), "parameters.txt"), "wb") as fh:
+        fh.write(released[tag + "|parameters"].tobytes())
+    return prefix, entries
 
 
 def test_crc32c_known_answers():
@@ -48,6 +69,25 @@ def test_bundle_round_trip(tmp_path):
         ck.read_checkpoint(prefix, names=["nope"])
 
 
+def test_load_params_keeps_model_variables_only(tmp_path):
+    """load_params: the variables under the model scope, keyed without it; optimizer slots (every kind the reference's
+    optimizers write), counters and variables outside the scope are dropped."""
+    w = np.arange(6, dtype=np.float32).reshape(2, 3)
+    tensors = {ck.MODEL_SCOPE + "layer_0/simple_0/weights": w,
+               ck.MODEL_SCOPE + "layer_0/simple_0/bn/moving_mean": np.ones(3, np.float32),
+               "global_step": np.array(3, np.int64), "beta1_power": np.array(0.9, np.float32),
+               "other_scope/layer_0/weights": np.zeros(2, np.float32)}
+    for slot in ck._OPTIMIZER_SLOTS:
+        tensors[ck.MODEL_SCOPE + "layer_0/simple_0/weights" + slot] = np.zeros_like(w)
+    prefix = str(tmp_path / "snap-3")
+    ck.write_checkpoint(prefix, tensors)
+    params = ck.load_params(prefix)
+    assert set(params) == {"layer_0/simple_0/weights", "layer_0/simple_0/bn/moving_mean"}
+    assert np.array_equal(params["layer_0/simple_0/weights"], w)
+    with pytest.raises(ck.CheckpointError, match="no variables"):
+        ck.load_params(prefix, scope="Missing/")
+
+
 def test_bundle_corruption_is_detected(tmp_path):
     prefix = str(tmp_path / "snap-2")
     ck.write_checkpoint(prefix, {"a/b": np.arange(10, dtype=np.float32)})
@@ -66,35 +106,43 @@ def test_bundle_corruption_is_detected(tmp_path):
         ck.read_index(prefix)
 
 
-@needs_ref
-def test_released_snapshots_known_answers():
-    log = os.path.join(REF, "results_kitti", "Log_11011605")
-    params = ck.load_params(os.path.join(log, "snapshots", "snap-61"))
-    plys = sorted(glob.glob(os.path.join(log, "kernel_points", "epoch61", "*.ply")))
+def test_released_snapshots_known_answers(released, tmp_path):
+    kp_names = sorted(k[len("kitti61|data|"):] for k in released if k.startswith("kitti61|data|"))
+    assert len(kp_names) == 10
+    prefix, _ = released_snapshot(released, "kitti61", 61, tmp_path, kp_names)
+    params = ck.read_checkpoint(prefix, names=kp_names)
+    plys = sorted(k[len("kitti61|ply|"):] for k in released if k.startswith("kitti61|ply|"))
     assert len(plys) == 10
-    for f in plys:
-        base = os.path.basename(f)[:-4]                                      # layer_1_resnetb_0_conv2
-        names = [n for n in params if n.endswith("kernel_points") and n.replace("/", "_").startswith(base + "_k")]
+    for base in plys:                                                        # layer_1_resnetb_0_conv2
+        names = [n for n in params if n[len(ck.MODEL_SCOPE):].replace("/", "_").startswith(base + "_k")]
         assert len(names) == 1, base
-        want = io_utils.read_ply_points(f)
+        f = tmp_path / (base + ".ply")
+        released["kitti61|ply|" + base].tofile(str(f))
+        want = io_utils.read_ply_points(str(f))
         assert np.array_equal(params[names[0]].view(np.uint32), want.view(np.uint32)), base
     # variable names / shapes == what the host mirror asks for, for every released model
-    for log, snap in (("results_kitti/Log_11011605", 61), ("results/Log_contraloss", 54), ("results/Log_circleloss", 48)):
-        cfg = io_utils.load_config(os.path.join(REF, log))
-        got = ck.load_params(os.path.join(REF, log, "snapshots", "snap-%d" % snap))
+    for tag, snap in RELEASED:
+        prefix, entries = released_snapshot(released, tag, snap, tmp_path / "names")
+        cfg = io_utils.load_config(os.path.dirname(prefix))
+        got = {n[len(ck.MODEL_SCOPE):]: e for n, e in entries.items()
+               if n.startswith(ck.MODEL_SCOPE) and not n.endswith(ck._OPTIMIZER_SLOTS)}
         want = synth.make_params(cfg, 0)
-        assert set(got) == set(want), log
-        assert all(got[k].shape == tuple(np.shape(want[k])) and got[k].dtype == np.float32 for k in got), log
+        assert set(got) == set(want), tag
+        assert all(tuple(got[k]["shape"]) == tuple(np.shape(want[k])) and got[k]["dtype"] == 1 for k in got), tag
         assert cfg.num_layers == 5 and cfg.first_features_dim == 64 and cfg.num_kernel_points == 15
 
 
-@needs_ref
-def test_config_and_ply_readers_on_reference_files():
-    cfg = io_utils.load_config(os.path.join(REF, "results", "Log_contraloss"))
+def test_config_and_ply_readers_on_reference_files(released, tmp_path):
+    prefix, _ = released_snapshot(released, "contraloss54", 54, tmp_path)
+    cfg = io_utils.load_config(os.path.dirname(prefix))
     assert cfg.architecture[0] == "simple" and cfg.architecture[-1] == "last_unary" and len(cfg.architecture) == 19
     assert abs(cfg.first_subsampling_dl - 0.03) < 1e-9 and cfg.KP_influence == "linear" and cfg.modulated is False
-    pts = io_utils.read_ply_points(os.path.join(REF, "demo_data", "cloud_bin_0.ply"))
-    assert pts.shape == (258342, 3) and pts.dtype == np.float32 and np.isfinite(pts).all()
+    # the demo scan's binary PLY (CloudCompare header, comments, obj_info), cut to its first 2000 vertices
+    f = tmp_path / "cloud_bin_0.ply"
+    released["demo|cloud_bin_0_head"].tofile(str(f))
+    pts = io_utils.read_ply_points(str(f))
+    assert pts.shape == (2000, 3) and pts.dtype == np.float32 and np.isfinite(pts).all()
+    assert np.array_equal(pts.view(np.uint32), released["demo|cloud_bin_0_points"].view(np.uint32))
 
 
 def test_ply_ascii_and_big_endian(tmp_path):
@@ -129,41 +177,3 @@ def test_keypoint_selection_and_writers(tmp_path):
     assert d.shape == (N, 32) and k.shape == (N, 3) and s.shape == (N, 1) and d.dtype == np.float32
     assert (np.diff(s[:, 0]) >= 0).all()                    # ascending: evaluate.py takes the LAST 250 rows
     assert np.array_equal(k[-1], pts[np.argmax(sc)]) and np.array_equal(d[-1], desc[np.argmax(sc)])
-
-
-@needs_ref
-def test_released_model_registers_the_demo_pair_through_the_restatement():
-    """Behavioural known answer for the TF-graph restatement (oracle/kpconv_np.py): with the RELEASED 3DMatch weights,
-    BN statistics and kernel points (read by tf_checkpoint.py) the numpy encoder + decoder + detector must produce
-    descriptors that register the reference's demo fragments (demo_registration.py flow); with the weights shuffled
-    inside each tensor the matches must collapse. scripts/oracle_released_demo.py is the full-size version
-    (2500 keypoints: 53 % inlier ratio, overlap 6 % -> 81 %, tests/golden/released_demo_summary.json)."""
-    import importlib.util
-    from scipy.spatial import cKDTree
-    from oracle import native as on
-    spec = importlib.util.spec_from_file_location(
-        "oracle_released_demo", os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "scripts",
-                                             "oracle_released_demo.py"))
-    demo = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(demo)
-    if not on.have_ref():
-        on.build(ref=True)
-    cfg = io_utils.load_config(os.path.join(REF, "results", "Log_contraloss"))
-    params = ck.load_params(os.path.join(REF, "results", "Log_contraloss", "snapshots", "snap-54"))
-    clouds = []
-    for i in (0, 1):
-        raw = io_utils.read_ply_points(os.path.join(REF, "demo_data", "cloud_bin_%d.ply" % i))
-        clouds.append(on.ref_batch_subsampling(raw, np.array([raw.shape[0]], np.int32), cfg.first_subsampling_dl)[0])
-    limits = [37, 35, 36, 38, 38]                       # demo.calibrate(cfg, clouds), tests/golden/released_demo_summary.json
-    d, s = zip(*(demo.describe(cfg, params, limits, c) for c in clouds))
-    assert all(np.allclose(np.linalg.norm(x, axis=1), 1.0, atol=1e-4) for x in d)
-    kp = [np.argsort(x[:, 0])[-1500:] for x in s]
-    d0, d1 = d[0][kp[0]], d[1][kp[1]]
-    nn01 = cKDTree(d1).query(d0)[1]
-    mutual = np.nonzero(cKDTree(d0).query(d1)[1][nn01] == np.arange(d0.shape[0]))[0]
-    src, dst = clouds[0][kp[0]][mutual], clouds[1][kp[1]][nn01[mutual]]
-    r, t, inl = demo.ransac(src, dst, iters=3000)
-    assert mutual.size > 100 and inl.sum() / mutual.size > 0.3
-    before = np.mean(cKDTree(clouds[1]).query(clouds[0])[0] < 0.05)
-    after = np.mean(cKDTree(clouds[1]).query(clouds[0] @ r.T + t)[0] < 0.05)
-    assert before < 0.15 and after > 0.6

@@ -254,7 +254,7 @@ def test_deformable_architecture_runs_and_matches(cuda):
                                           (3600, 3600, 8, 32)])
 def test_kpconv_fused_kernel_matches_restatement_and_two_kernel_path(cuda, monkeypatch, Nq, Ns, H, Cout):
     """The persistent fused kernel of the Cin = 32 layers (kpconv_fused.cu: gather + correlation on mma.sync, contraction
-    on tcgen05 out of a shared-memory A operand): vs the float64 restatement (1e-4) and vs the two-kernel path of the
+    on wgmma out of a shared-memory B operand): vs the float64 restatement (1e-4) and vs the two-kernel path of the
     same library (both 3xTF32: agree far below the tolerance). Ragged tail tile (Nq % 48 != 0), strided queries
     (Nq != Ns), H not a multiple of 8, fused BN + LeakyReLU epilogue."""
     from d3feat_b200 import convolution_ops as co

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 (3xTF32, TMEM accumulator) GEMM path vs float64, and vs the CUDA-core fp32 path."""
+"""GPU: the wgmma (3xTF32, register accumulator) GEMM path vs float64, and vs the CUDA-core fp32 path."""
 import numpy as np
 import pytest
 import torch
@@ -30,8 +30,8 @@ def test_tc_gemm_matches_float64(cuda, monkeypatch, M, K, N):
     monkeypatch.setattr(co, "USE_TENSOR_CORES", False)
     out_cc = co.unary_convolution(tx, tw).cpu().numpy()
     e_tc, e_cc = rel_err(out_tc, ref), rel_err(out_cc, ref)
-    # 3xTF32 keeps ~21 mantissa bits per product; what remains is the tensor pipe's truncating fp32 accumulate
-    # (~1.1e-8 * K / kAcc relative, measured by scripts/tc_accuracy_probe.py): 1.4e-5 at K = 7680, inside the 1e-4 budget
+    # 3xTF32 keeps ~21 mantissa bits per product; the tensor pipe's own accumulate is restarted every 32-wide k-chunk
+    # and the chunks are summed with round-to-nearest (tc_gemm.cu)
     assert e_tc < 3e-5, (e_tc, e_cc)
     assert e_cc < 1e-5, (e_tc, e_cc)
 
@@ -103,9 +103,8 @@ def test_unary_pair_convolution(cuda, N, C1, C2, Cout):
 @pytest.mark.parametrize("stream", [0, 1])
 def test_streaming_gemm_large_m(cuda, monkeypatch, M, K, N, stream):
     """Huge-M GEMMs vs float64, through the default one-tile-per-CTA kernels (stream = 0) and through the opt-in
-    persistent streaming variant (D3F_TC_STREAM=1: tc_gemm_stream_kernel takes the GEMMs with >= 296 output tiles,
-    K >= 256 and a column tile <= 64 -- transposed single-MMA product, ring running across tiles, double-buffered TMEM,
-    separate epilogue warps). Ragged last tile, partial column tile (N = 48), BN + LeakyReLU + residual epilogue,
+    persistent launch (D3F_TC_STREAM=1: one CTA per SM walks several tiles, the operand ring running across
+    tiles). Ragged last tile, partial column tile (N = 48), BN + LeakyReLU + residual epilogue,
     several n-tiles per row block, and a device-side row count below the launch capacity."""
     from d3feat_b200 import convolution_ops as co
     monkeypatch.setattr(co, "USE_TENSOR_CORES", True)

@@ -94,7 +94,7 @@ def test_calibrate_neighbors_matches_oracle_counts(cuda):
 
 def test_config3_full_size_deformable(cuda, monkeypatch):
     """BASELINE.json configs[2]: one 120k-point KITTI-shaped scan through the deformable architecture. Too large for
-    the numpy restatement, so the check is the size-independent one: the tcgen05 3xTF32 path and the independent
+    the numpy restatement, so the check is the size-independent one: the wgmma 3xTF32 path and the independent
     CUDA-core fp32 path (each pinned to the restatement at small sizes) agree to 1e-4 on every level, the pyramid
     is well-formed, and a second run is bit-identical (no atomics on float data)."""
     from d3feat_b200 import synth

@@ -1,5 +1,6 @@
 """CPU: pin the oracle (C restatement) to the golden vectors generated from the reference's own compiled
-C++ cores (scripts/make_golden.py) and, when oracle/_ref is present, to those cores directly."""
+C++ cores (scripts/make_golden.py, scripts/make_golden_ref_digests.py) and, when oracle/_ref is present, to those
+cores directly."""
 import numpy as np
 import pytest
 
@@ -88,20 +89,36 @@ def test_ordered_neighbors_vs_golden(golden):
     assert (g["ord_neighbors"] == -1).any()
 
 
-@pytest.mark.skipif(not on.have_ref(), reason="oracle/_ref not built (no /root/reference here)")
-def test_port_vs_compiled_reference_random():
+def digest(a):
+    import hashlib
+    a = np.ascontiguousarray(a)
+    return dict(shape=list(a.shape), dtype=str(a.dtype), sha256=hashlib.sha256(a.tobytes()).hexdigest())
+
+
+def test_port_vs_compiled_reference_random(golden_json):
+    """The C port vs what the reference's compiled cores returned on the same seeded clouds (digests of the canonical
+    forms, scripts/make_golden_ref_digests.py), and vs those cores directly when oracle/_ref is present."""
+    want = golden_json("reference_digests.json")["random_trials"]
     rng = np.random.default_rng(0)
     for trial in range(3):
         n1, n2 = rng.integers(200, 1500, 2)
         P = rng.uniform(-1, 1, (n1 + n2, 3)).astype(np.float32)
         L = np.array([n1, n2], np.int32)
         r = float(rng.uniform(0.1, 0.3))
-        ref = on.ref_batch_neighbors(P, P, L, L, r)
-        canon, _ = on.canonicalize_neighbors(ref, P, P, P.shape[0])
-        assert np.array_equal(on.port_batch_neighbors(P, P, L, L, r), canon)
-        rp, rb = on.ref_batch_subsampling(P, L, r)
+        nb = on.port_batch_neighbors(P, P, L, L, r)
+        assert digest(nb.astype(np.int32)) == want[trial]["neighbors"]
         pp, pb = on.port_batch_subsampling(P, L, r)
-        per_cloud_sets_equal(pp, pb, rp, rb)
+        assert pb.tolist() == want[trial]["subsampling"]["lengths"]
+        o = 0
+        for n, w in zip(pb, want[trial]["subsampling"]["clouds"]):
+            assert digest(on.sort_rows(bits(pp[o:o + n]))[0]) == w
+            o += n
+        if on.have_ref():
+            ref = on.ref_batch_neighbors(P, P, L, L, r)
+            canon, _ = on.canonicalize_neighbors(ref, P, P, P.shape[0])
+            assert np.array_equal(nb, canon)
+            rp, rb = on.ref_batch_subsampling(P, L, r)
+            per_cloud_sets_equal(pp, pb, rp, rb)
 
 
 def test_empty_and_single_point_inputs():
