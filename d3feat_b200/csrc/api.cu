@@ -129,7 +129,8 @@ int d3f_kpconv_forward(const float* q, const float* s, const int* idx, const flo
                        int mode, int normalize, const float* bn_scale, const float* bn_shift, const float* bias,
                        float leaky_alpha, float* out, void* workspace, size_t workspace_bytes, d3f_stream_t stream,
                        const int* nq_dev, const int* ns_dev) {
-  D3F_REQUIRE(Nq == 0 || (q && s && idx && feat && Kp && W && out && workspace), D3F_ERR_INVALID,
+  // an empty support set (Ns == 0: every index is the shadow point) has no coordinates or features to point at
+  D3F_REQUIRE(Nq == 0 || (q && idx && Kp && W && out && workspace && (Ns == 0 || (s && feat))), D3F_ERR_INVALID,
               "d3f_kpconv_forward: null pointer");
   return kpconv_forward_impl(false, q, s, idx, feat, Kp, nullptr, nullptr, W, W_packed, query_order, Nq, Ns, H, K, Cin, Cout, extent,
                              influence, mode, normalize, bn_scale, bn_shift, bias, leaky_alpha, out, workspace,
@@ -142,8 +143,8 @@ int d3f_kpconv_deform_forward(const float* q, const float* s, const int* idx, co
                               const float* bn_shift, const float* bias, float leaky_alpha, float* out,
                               void* workspace, size_t workspace_bytes, d3f_stream_t stream, const int* nq_dev,
                               const int* ns_dev) {
-  D3F_REQUIRE(Nq == 0 || (q && s && idx && feat && Kp && W && out && workspace && offsets), D3F_ERR_INVALID,
-              "d3f_kpconv_deform_forward: null pointer");
+  D3F_REQUIRE(Nq == 0 || (q && idx && Kp && W && out && workspace && offsets && (Ns == 0 || (s && feat))),
+              D3F_ERR_INVALID, "d3f_kpconv_deform_forward: null pointer");
   return kpconv_forward_impl(true, q, s, idx, feat, Kp, offsets, modulations, W, W_packed, query_order, Nq, Ns, H, K, Cin, Cout, extent,
                              influence, mode, 0, bn_scale, bn_shift, bias, leaky_alpha, out, workspace,
                              workspace_bytes, (cudaStream_t)stream, nq_dev, ns_dev);

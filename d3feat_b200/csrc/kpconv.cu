@@ -953,10 +953,9 @@ static int launch_stage1(int K, const Stage1Params& p, cudaStream_t stream) {
     D3F_LAUNCH_CHECK("kpconv_stage1_mma_kernel");
     return D3F_OK;
   }
-  // (channels per lane, queries per warp): every broadcast weight read should feed as much math as possible
-  if (K == 15 && al16 && p.Cin % 128 == 0) {
-    kpconv_stage1_v2_kernel<4, 1, DEFORM><<<ceil_div(nq, kS1Warps), kS1Warps * 32, 0, stream>>>(p);
-  } else if (K == 15 && al16 && p.Cin % 64 == 0) {
+  // (channels per lane, queries per warp): every broadcast weight read should feed as much math as possible.
+  // Cin % 128 == 0 never gets here (taken by the tensor-core kernels above), so CPL = 2 is the widest instance.
+  if (K == 15 && al16 && p.Cin % 64 == 0) {
     kpconv_stage1_v2_kernel<2, 1, DEFORM><<<ceil_div(nq, kS1Warps), kS1Warps * 32, 0, stream>>>(p);
   } else if (K == 15 && al16 && p.Cin % 32 == 0) {
     kpconv_stage1_v2_kernel<2, 2, DEFORM><<<ceil_div(nq, kS1Warps * 2), kS1Warps * 32, 0, stream>>>(p);
@@ -1172,7 +1171,7 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
               "Unknown convolution mode. Should be 'closest' or 'sum'");
   D3F_REQUIRE(extent > 0.f, D3F_ERR_INVALID, "kpconv: KP_extent=%g", (double)extent);
   D3F_REQUIRE((bn_scale == nullptr) == (bn_shift == nullptr), D3F_ERR_INVALID, "kpconv: bn_scale/bn_shift mismatch");
-  D3F_REQUIRE(!deform || offsets != nullptr, D3F_ERR_INVALID, "kpconv_deform: offsets missing");
+  D3F_REQUIRE(!deform || offsets != nullptr || Nq == 0, D3F_ERR_INVALID, "kpconv_deform: offsets missing");
   D3F_REQUIRE(workspace_bytes >= kpconv_workspace_bytes(Nq, Ns, H, K, Cin, Cout), D3F_ERR_WORKSPACE,
               "kpconv: workspace too small");
   if (Nq == 0) return D3F_OK;

@@ -25,12 +25,28 @@ def unary_convolution(features, K_values):
     return features @ K_values
 
 
+# Discontinuities of the graph that fp32 and fp64 may legitimately resolve differently (magnitude=True marks them):
+CLOSEST_TIE_RTOL = 1e-5            # closest mode: the two nearest kernel points' d2 differ by less than this, relative
+NN_SUM_ULPS = 64 * 2.0 ** -24      # nn predicate: |row sum| < this * sum |row| (a float64 sum of exactly 0 is exact)
+IN_RANGE_RTOL = 1e-5               # deformable in-range / constant weight: |d2 - extent^2| < this * extent^2
+
+
+
 def kpconv_ops(query_points, support_points, neighbors_indices, features, K_points, K_values, KP_extent,
-               KP_influence="linear", aggregation_mode="sum", dtype=np.float64, chunk=2048):
+               KP_influence="linear", aggregation_mode="sum", dtype=np.float64, chunk=2048, magnitude=False):
     """kernels/convolution_ops.py:161-255 (KPConv_ops), steps 1-11 of SURVEY.md section 3.2.
 
     dtype=np.float64 evaluates the same graph in double (the tolerance oracle); np.float32 mimics the
     reference's arithmetic type (summation order of tf.matmul / reduce_sum is not reproducible).
+
+    magnitude=True returns (out, mag, alt):
+      mag  the same contraction on absolute values, sum_k w^T |f| @ |W_k| / nn (the influence weights are
+           non-negative; nn is counted on the SIGNED features), the scale of the rounding error of any
+           summation order of out, per element;
+      alt  out with every ambiguous decision taken the other way: a closest-mode neighbour whose two nearest
+           kernel points are tied within CLOSEST_TIE_RTOL goes to the second one, a support whose feature-row sum
+           is within NN_SUM_ULPS of zero (but not exactly zero) flips its nn vote. alt == out on rows without
+           such a decision; mag covers both branches.
     """
     if KP_influence not in INFLUENCES:
         raise ValueError("Unknown influence function type (config.KP_influence)")
@@ -48,6 +64,8 @@ def kpconv_ops(query_points, support_points, neighbors_indices, features, K_poin
     n_kp = Kp.shape[0]
     Nq = q.shape[0]
     out = np.zeros((Nq, W.shape[2]), dt)
+    if magnitude:
+        mag, alt, mag_alt = np.zeros_like(out), np.zeros_like(out), np.zeros_like(out)
     ext = dt(KP_extent)
     for a, b in _chunks(Nq, chunk):
         ii = idx[a:b]
@@ -62,6 +80,7 @@ def kpconv_ops(query_points, support_points, neighbors_indices, features, K_poin
             sigma = ext * dt(0.3)                                      # :218-222, radius_gaussian :48-55
             w = np.exp(-d2 / (2 * np.square(sigma) + dt(1e-9)))
         w = np.transpose(w, (0, 2, 1))                                 # [n,K,H]
+        w_all = w
         if aggregation_mode == "closest":                              # :227-229
             nn1 = np.argmin(d2, axis=2)                                # [n,H]
             onehot = (np.arange(n_kp)[None, :, None] == nn1[:, None, :]).astype(dt)
@@ -73,17 +92,39 @@ def kpconv_ops(query_points, support_points, neighbors_indices, features, K_poin
         nnum = np.sum((nsum > 0).astype(dt), axis=-1)                  # :251
         nnum = np.maximum(nnum, 1)                                     # :252
         out[a:b] = ko / nnum[:, None]                                  # :253
+        if not magnitude:
+            continue
+        aW = np.abs(W)
+        mag[a:b] = np.einsum("nkc,kco->no", np.matmul(w, np.abs(nf)), aW) / nnum[:, None]
+        w2 = w
+        if aggregation_mode == "closest" and n_kp > 1:
+            srt = np.sort(d2, axis=2)
+            tie = srt[:, :, 1] - srt[:, :, 0] <= CLOSEST_TIE_RTOL * srt[:, :, 1]
+            second = np.argsort(d2, axis=2, kind="stable")[:, :, 1]
+            nn2 = np.where(tie, second, nn1)
+            w2 = w_all * (np.arange(n_kp)[None, :, None] == nn2[:, None, :]).astype(dt)
+        asum = np.sum(np.abs(nf), axis=-1)
+        amb = (nsum != 0) & (np.abs(nsum) < NN_SUM_ULPS * asum)
+        nnum2 = np.maximum(np.sum(((nsum > 0) ^ amb).astype(dt), axis=-1), 1)
+        alt[a:b] = np.einsum("nkc,kco->no", np.matmul(w2, nf), W) / nnum2[:, None]
+        mag_alt[a:b] = np.einsum("nkc,kco->no", np.matmul(w2, np.abs(nf)), aW) / nnum2[:, None]
+    if magnitude:
+        return out, np.maximum(mag, mag_alt), alt
     return out
 
 
 def kpconv_deform_ops(query_points, support_points, neighbors_indices, features, K_points, offsets,
                       modulations, K_values, KP_extent, KP_influence="linear", mode="sum",
-                      dtype=np.float64, chunk=1024):
+                      dtype=np.float64, chunk=1024, magnitude=False):
     """kernels/convolution_ops.py:379-499 (KPConv_deform_ops).
 
     The top_k compaction (:435-451) is restated as its net effect: a neighbour that is in range of no
     deformed kernel point is re-pointed to the shadow row (zero features); the kept ones keep their
     sq_distances. No neighbour-count normalisation in this op.
+
+    magnitude=True returns (out, mag, alt) as kpconv_ops does (modulations are positive, so they enter mag as
+    they are); the ambiguous decisions here are the closest-mode ties and every d2 < extent^2 comparison with
+    |d2 - extent^2| < IN_RANGE_RTOL * extent^2 (the in-range test and the constant influence).
     """
     if KP_influence not in INFLUENCES:
         raise ValueError("Unknown influence function type (config.KP_influence)")
@@ -101,29 +142,51 @@ def kpconv_deform_ops(query_points, support_points, neighbors_indices, features,
     Nq = q.shape[0]
     ext = dt(KP_extent)
     out = np.zeros((Nq, W.shape[2]), dt)
+    if magnitude:
+        mag, alt = np.zeros_like(out), np.zeros_like(out)
     for a, b in _chunks(Nq, chunk):
         ii = idx[a:b]
         nb = s[ii] - q[a:b, None, :]                                   # :417-420
         dKp = off[a:b] + Kp[None]                                      # :424      [n,K,3]
         diff = nb[:, :, None, :] - dKp[:, None, :, :]                  # :427-429  [n,H,K,3]
         d2 = np.sum(np.square(diff), axis=3)                           # :432
-        in_range = np.any(d2 < ext ** 2, axis=2)                       # :435      [n,H]
-        if KP_influence == "constant":
-            w = (d2 < ext ** 2).astype(dt)                             # :456
-        elif KP_influence == "linear":
-            w = np.maximum(1 - np.sqrt(d2 + dt(1e-10)) / ext, dt(0.0))  # :461 (no factor 2)
-        else:
-            sigma = ext * dt(0.3)
-            w = np.exp(-d2 / (2 * np.square(sigma) + dt(1e-9)))
-        w = np.transpose(w, (0, 2, 1))
-        if mode == "closest":
-            nn1 = np.argmin(d2, axis=2)
-            w = w * (np.arange(n_kp)[None, :, None] == nn1[:, None, :]).astype(dt)
-        nf = f[ii] * in_range[:, :, None].astype(dt)                   # :441-451, 483
-        wf = np.matmul(w, nf)                                          # :486
-        if modulations is not None:
-            wf = wf * np.asarray(modulations, dt)[a:b, :, None]        # :489-490
-        out[a:b] = np.einsum("nkc,kco->no", wf, W)                     # :493-497
+        mod = None if modulations is None else np.asarray(modulations, dt)[a:b, :, None]
+
+        def contract(inside, nn1, feats):
+            in_range = np.any(inside, axis=2)                          # :435      [n,H]
+            if KP_influence == "constant":
+                w = inside.astype(dt)                                  # :456
+            elif KP_influence == "linear":
+                w = np.maximum(1 - np.sqrt(d2 + dt(1e-10)) / ext, dt(0.0))  # :461 (no factor 2)
+            else:
+                sigma = ext * dt(0.3)
+                w = np.exp(-d2 / (2 * np.square(sigma) + dt(1e-9)))
+            w = np.transpose(w, (0, 2, 1))
+            if mode == "closest":
+                w = w * (np.arange(n_kp)[None, :, None] == nn1[:, None, :]).astype(dt)
+            nf = feats * in_range[:, :, None].astype(dt)               # :441-451, 483
+            wf = np.matmul(w, nf)                                      # :486
+            if mod is not None:
+                wf = wf * mod                                          # :489-490
+            return wf
+
+        inside = d2 < ext ** 2
+        nn1 = np.argmin(d2, axis=2)
+        out[a:b] = np.einsum("nkc,kco->no", contract(inside, nn1, f[ii]), W)   # :493-497
+        if not magnitude:
+            continue
+        near = np.abs(d2 - ext ** 2) < IN_RANGE_RTOL * ext ** 2
+        nn2 = nn1
+        if mode == "closest" and n_kp > 1:
+            srt = np.sort(d2, axis=2)
+            tie = srt[:, :, 1] - srt[:, :, 0] <= CLOSEST_TIE_RTOL * srt[:, :, 1]
+            nn2 = np.where(tie, np.argsort(d2, axis=2, kind="stable")[:, :, 1], nn1)
+        aW = np.abs(W)
+        alt[a:b] = np.einsum("nkc,kco->no", contract(inside ^ near, nn2, f[ii]), W)
+        mag[a:b] = np.maximum(np.einsum("nkc,kco->no", contract(inside, nn1, np.abs(f[ii])), aW),
+                              np.einsum("nkc,kco->no", contract(inside ^ near, nn2, np.abs(f[ii])), aW))
+    if magnitude:
+        return out, mag, alt
     return out
 
 

@@ -150,15 +150,55 @@ def test_bench_workload_every_op_sampled_rows_vs_float64(cuda, bench_workload):
         out = enc(P, L, decoder=False)
         torch.cuda.synchronize()
     assert out["F"][-1].shape[1] == 2048
-    rep = check_sampled_rows(tr, 2000, np.random.default_rng(0), RTOL, min_kpconv=10)
+    rep = check_sampled_rows(tr, 2000, np.random.default_rng(0), RTOL, min_kpconv=10, what="bench exact")
     assert sum(1 for r in rep if r[0] in ("unary", "unary_pair")) >= 18
-    # the single-shot result equals the pipelined one bit for bit (BatchPipeline is what bench.py times)
+    # the single-shot result equals the eager two-stream pipeline's bit for bit (BatchPipeline, bench.py --no-graph;
+    # the default timed path, GraphPipeline, is checked by test_bench_timed_path_static_pyramid_vs_float64)
     from d3feat_b200.encoder import BatchPipeline
     pipe = BatchPipeline(enc, decoder=False)
     pipe.prime(t(P, cuda), t(L, cuda))
     res = pipe.step(None, None)
     pipe.drain()
     assert torch.equal(res, out["F"][-1])
+
+
+def test_bench_timed_path_static_pyramid_vs_float64(cuda, bench_workload):
+    """What bench.py times by default, at its shape: the static pyramid (capacity-sized launches, level sizes only in
+    device memory) sized as GraphPipeline.for_batch sizes it, the encoder run eagerly on it with every op's float64
+    restatement checked on 2000 sampled rows below the device count; then GraphPipeline with bench.py's two encoder
+    streams, stepped twice on the same batch, returns the eager static result bit for bit (same kernels, same
+    capacity plan)."""
+    from d3feat_b200 import pyramid as pyr
+    from d3feat_b200.encoder import GraphPipeline
+    cfg, params, clouds, P, L, enc = bench_workload
+    Pd, Ld = t(P, cuda), t(L, cuda)
+    pipe = GraphPipeline.for_batch(enc, Pd, Ld, decoder=False, encoder_streams=2)
+    buf = pyr.PyramidBuffers(cfg, enc.limits, pipe.caps, pipe.n_clouds, cuda, bbox=pipe.bbox)
+    n0 = P.shape[0]
+    buf.points0[:n0].copy_(Pd)
+    buf.lengths0.copy_(Ld)
+    buf.n0.fill_(n0)
+    inputs = enc.build_inputs_static(buf)
+    with record_ops() as tr:
+        F = enc.encode(inputs)
+        torch.cuda.synchronize()
+    assert int(inputs["status"].item()) == 0
+    counts = inputs["counts"][:5].cpu().tolist()
+    assert all(0 < c <= cap for c, cap in zip(counts, pipe.caps)) and int(F[-1].shape[0]) >= counts[4]
+    assert all(r.get("rows_q") is not None for r in tr.records)      # every op ran capacity-sized
+    rep = check_sampled_rows(tr, 2000, np.random.default_rng(2), RTOL, min_kpconv=10, what="bench static")
+    assert sum(1 for r in rep if r[0] in ("unary", "unary_pair")) >= 18
+    print("bench static path: largest |err|/mag over %d ops: %.3e" % (len(rep), max(r[3] for r in rep)))
+    eager = F[-1][:counts[4]].clone()
+    pipe.prime(Pd, Ld)
+    got = []
+    for i in range(2):
+        res, cnt = pipe.step(Pd, Ld) if i == 0 else pipe.step()
+        got.append((res.clone(), cnt.clone()))
+    pipe.check()
+    for res, cnt in got:
+        assert cnt[:5].cpu().tolist() == counts
+        assert torch.equal(res[:counts[4]], eager)
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -241,7 +281,7 @@ def test_kitti_120k_every_op_sampled_rows_vs_float64(cuda):
     nb_fn, sb_fn, which = oracle_native_fns()
     ref = ok.descriptor_input_pyramid(cfg, cloud, L, limits, nb_fn, sb_fn)
     assert_pyramid_equal(inputs, ref, len(ref["points"]))
-    rep = check_sampled_rows(tr, 2000, np.random.default_rng(1), RTOL, min_kpconv=10)
+    rep = check_sampled_rows(tr, 2000, np.random.default_rng(1), RTOL, min_kpconv=10, what="kitti 120k")
     assert any(r[0] == "kpconv_deform" for r in rep)
     # reproducible: no atomics on float data anywhere on the path
     F2 = enc(cloud, L)["F"]

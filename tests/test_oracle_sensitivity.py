@@ -1,0 +1,168 @@
+"""The element-wise check (tests/_oracle.py) is tight enough to matter: it rejects numpy emulations of the ways a KPConv
+or GEMM kernel typically goes wrong, at the shapes of the GPU tests, and accepts the float32 evaluation of the same
+restatement (what an honest fp32 kernel with another summation order computes). No GPU needed."""
+import numpy as np
+import pytest
+
+from oracle import kpconv_np as ok
+
+from _oracle import TOL, assert_close, gemm_mag, epilogue, tf32, f64
+from test_gpu_kpconv import make_case
+
+
+def rejects(out, ref, mag, alt=None):
+    with pytest.raises(AssertionError):
+        assert_close(out, ref, mag, TOL, "emulated bug", alt=alt)
+
+
+# ---- GEMM (unary convolution, and the KPConv contraction [Nq, K*Cin] @ [K*Cin, Cout]) --------------------------------
+
+GEMM_SHAPES = [(3000, 64, 32), (3000, 32, 128), (645, 1024, 256), (700, 960, 64)]
+
+
+def _gemm_case(N, Cin, Cout):
+    rng = np.random.default_rng(N + Cin + Cout)
+    x = rng.normal(size=(N, Cin)).astype(np.float32)
+    w = (rng.normal(size=(Cin, Cout)) * np.sqrt(2.0 / Cout)).astype(np.float32)
+    return x, w, f64(x) @ f64(w), gemm_mag(x, w)
+
+
+@pytest.mark.parametrize("N,Cin,Cout", GEMM_SHAPES)
+def test_float32_gemm_is_accepted(N, Cin, Cout):
+    x, w, ref, mag = _gemm_case(N, Cin, Cout)
+    assert_close(x @ w, ref, mag, TOL, "fp32 gemm %dx%dx%d" % (N, Cin, Cout))
+    rng = np.random.default_rng(1)
+    scale = rng.uniform(0.5, 1.5, Cout).astype(np.float32)
+    shift = rng.normal(size=Cout).astype(np.float32)
+    res = rng.normal(size=(N, Cout)).astype(np.float32)
+    y, m = epilogue(ref, mag, scale, shift, residual=res, alpha=0.2)
+    y32 = (x @ w) * scale + shift + res
+    y32 = np.where(y32 > 0, y32, np.float32(0.2) * y32)
+    assert_close(y32, y, m, TOL, "fp32 gemm + epilogue")
+
+
+@pytest.mark.parametrize("N,Cin,Cout", GEMM_SHAPES)
+def test_one_pass_tf32_gemm_is_rejected(N, Cin, Cout):
+    x, w, ref, mag = _gemm_case(N, Cin, Cout)
+    rejects(tf32(x) @ tf32(w), ref, mag)
+
+
+@pytest.mark.parametrize("N,Cin,Cout", GEMM_SHAPES)
+def test_3xtf32_without_the_al_bh_term_is_rejected(N, Cin, Cout):
+    x, w, ref, mag = _gemm_case(N, Cin, Cout)
+    xh, wh = f64(tf32(x)), f64(tf32(w))
+    wl = f64(w) - wh
+    rejects(xh @ wh + xh @ wl, ref, mag)           # Ah.Bh + Ah.Bl; the Al.Bh correction is missing
+    xl = f64(x) - xh
+    assert_close(xh @ wh + xl @ wh + xh @ wl, ref, mag, TOL, "complete 3xTF32")
+
+
+@pytest.mark.parametrize("N,Cin,Cout", GEMM_SHAPES)
+def test_ragged_last_tile_left_at_zero_is_rejected(N, Cin, Cout):
+    x, w, ref, mag = _gemm_case(N, Cin, Cout)
+    assert N % 128 != 0
+    out = (x @ w).copy()
+    out[N // 128 * 128:] = 0
+    rejects(out, ref, mag)
+
+
+# ---- KPConv ---------------------------------------------------------------------------------------------------------
+
+KP_SHAPES = [(32, 32, 800, 800, 32, 0.1), (64, 64, 900, 3000, 37, 0.06), (48, 40, 500, 500, 40, 0.12)]
+
+
+def _kp_case(Cin, Cout, Nq, Ns, H, extent):
+    rng = np.random.default_rng(Cin * 7 + H)
+    q, s, idx, f, Kp, W = make_case(rng, Nq, Ns, H, Cin, Cout, extent=extent)
+    f[::5] = -np.abs(f[::5])          # some supports do not count towards nn
+    return q, s, idx, f, Kp, W
+
+
+def _nn(f, idx):
+    fs = np.concatenate([f.astype(np.float64), np.zeros((1, f.shape[1]))], 0)
+    return np.maximum((fs[idx].sum(-1) > 0).sum(-1), 1)
+
+
+@pytest.mark.parametrize("Cin,Cout,Nq,Ns,H,extent", KP_SHAPES)
+def test_kpconv_bugs_are_rejected_and_float32_accepted(Cin, Cout, Nq, Ns, H, extent):
+    q, s, idx, f, Kp, W = _kp_case(Cin, Cout, Nq, Ns, H, extent)
+    args = (Kp, W, extent, "linear", "sum")
+    ref, mag, alt = ok.kpconv_ops(q, s, idx, f, *args, dtype=np.float64, magnitude=True)
+    assert np.array_equal(ref, ok.kpconv_ops(q, s, idx, f, *args, dtype=np.float64))
+    out32 = ok.kpconv_ops(q, s, idx, f, *args, dtype=np.float32)
+    assert_close(out32, ref, mag, TOL, "fp32 kpconv Cin %d" % Cin, alt=alt)
+    # tensor-core operands rounded to TF32 once (1xTF32)
+    rejects(ok.kpconv_ops(q, s, idx, tf32(f), Kp, tf32(W), extent, "linear", "sum"), ref, mag, alt)
+    # one neighbour column skipped in one row: the real neighbour with the largest weight of row 7
+    r = 7
+    real = np.where(idx[r] < Ns)[0]
+    j = real[np.argmin(np.linalg.norm(s[idx[r, real]] - q[r], axis=1))]
+    idx_bug = idx.copy()
+    idx_bug[r, j] = Ns
+    rejects(ok.kpconv_ops(q, s, idx_bug, f, *args), ref, mag, alt)
+    # nn off by one in one row
+    nn = _nn(f, idx)
+    out = ref.copy()
+    out[r] *= nn[r] / (nn[r] + 1.0)
+    rejects(out, ref, mag, alt)
+    # two output rows swapped (a row map shifted by one slot)
+    out = ref.copy()
+    out[[10, 11]] = out[[11, 10]]
+    rejects(out, ref, mag, alt)
+    # ragged last tile of the contraction left at zero
+    out = ref.copy()
+    out[Nq // 128 * 128:] = 0
+    rejects(out, ref, mag, alt)
+
+
+@pytest.mark.parametrize("influence", ["constant", "linear", "gaussian"])
+@pytest.mark.parametrize("mode", ["sum", "closest"])
+def test_float32_accepted_every_influence_and_mode(influence, mode):
+    q, s, idx, f, Kp, W = _kp_case(32, 48, 800, 800, 32, 0.1)
+    ref, mag, alt = ok.kpconv_ops(q, s, idx, f, Kp, W, 0.1, influence, mode, magnitude=True)
+    out32 = ok.kpconv_ops(q, s, idx, f, Kp, W, 0.1, influence, mode, dtype=np.float32)
+    assert_close(out32, ref, mag, TOL, "fp32 kpconv %s %s" % (influence, mode), alt=alt)
+    rng = np.random.default_rng(3)
+    off = (rng.normal(size=(800, 15, 3)) * 0.03).astype(np.float32)
+    mods = rng.uniform(0.5, 1.5, (800, 15)).astype(np.float32)
+    ref, mag, alt = ok.kpconv_deform_ops(q, s, idx, f, Kp, off, mods, W, 0.1, influence, mode, magnitude=True)
+    out32 = ok.kpconv_deform_ops(q, s, idx, f, Kp, off, mods, W, 0.1, influence, mode, dtype=np.float32)
+    assert_close(out32, ref, mag, TOL, "fp32 deformable %s %s" % (influence, mode), alt=alt)
+    out = ref.copy()
+    out[5] *= 1.0 + 1e-3                                     # a 1e-3 slip in one row
+    rejects(out, ref, mag, alt)
+
+
+def test_nn_predicate_ambiguity_is_marked_but_exact_zero_rows_are_not():
+    """Rows summing to exactly zero ([a, -a, b, -b, ...], or all zero) are deterministic 'not > 0' in every summation
+    order and must not be marked; a row sum that is nonzero but within rounding of zero is marked (alt flips its nn
+    vote)."""
+    q, s, idx, f, Kp, W = _kp_case(32, 32, 400, 400, 24, 0.12)
+    used = np.unique(idx[idx < 400])
+    a, b, c = used[:3]
+    f[a] = 0
+    f[b, 0::2] = np.abs(f[b, 0::2])
+    f[b, 1::2] = -f[b, 0::2]                                  # exactly cancelling
+    ref, mag, alt = ok.kpconv_ops(q, s, idx, f, Kp, W, 0.12, "linear", "sum", magnitude=True)
+    assert np.array_equal(ref, alt)
+    f[c] = f[b]
+    f[c, 0] += np.float32(1e-6) * abs(f[c, 0])               # sum = tiny positive, far inside the rounding band
+    assert 0 < f64(f[c]).sum() < ok.NN_SUM_ULPS * np.abs(f64(f[c])).sum()
+    ref, mag, alt = ok.kpconv_ops(q, s, idx, f, Kp, W, 0.12, "linear", "sum", magnitude=True)
+    rows = np.any(idx == c, axis=1)
+    assert rows.any()
+    assert not np.array_equal(ref[rows], alt[rows])
+    assert np.array_equal(ref[~rows], alt[~rows])
+
+
+def test_closest_mode_ties_are_marked():
+    q, s, idx, f, Kp, W = _kp_case(32, 32, 400, 400, 24, 0.12)
+    Kp = Kp.copy()
+    # put a support exactly halfway between two kernel points of query 0 (in float32 input coordinates)
+    sup = int(idx[0, 0])
+    s = s.copy()
+    Kp[2] = Kp[1] + np.float32(0.02) * np.array([1, 0, 0], np.float32)
+    s[sup] = q[0] + (Kp[1] + Kp[2]) / 2
+    ref, mag, alt = ok.kpconv_ops(q, s, idx, f, Kp, W, 0.12, "linear", "closest", magnitude=True)
+    assert not np.array_equal(ref[0], alt[0])
+    assert np.array_equal(ref[1:], alt[1:]) or np.any(idx[1:] == sup)
