@@ -4,14 +4,19 @@
 //
 //   C[M,N] = epilogue( rowscale[m] * (A[M,K] @ W[K,N]) )
 //
-// * A is the activation matrix (row-major fp32 in global memory). It is loaded by 4 producer warps with coalesced
-//   16-byte cp.async copies, split into (hi, lo) in place and left in shared memory in the canonical K-major
-//   SWIZZLE_128B layout the wgmma descriptor expects (rows of 128 B = 32 fp32, 16-byte chunks XOR-ed with row%8).
-// * W is static: it is packed once (pack_weight_kernel) into K-major [Npad, Kpad] hi/lo images that arrive by TMA.
-// * Two consumer warpgroups issue the wgmmas (M = 64 rows each, N = BN, K = 8 per instruction); an mbarrier ring of
-//   3-4 stages overlaps the producers with the tensor pipe.
+// * A is the activation matrix (row-major fp32 in global memory). One producer thread loads each 128 x 32 k-chunk of
+//   it by TMA through a 2D tensor map (SWIZZLE_128B, out-of-bounds rows and columns zero-filled) into an mbarrier ring.
+// * W is static: it is packed once (pack_weight_kernel) into K-major [Npad, Kpad] hi/lo images that arrive by TMA bulk
+//   copies on the same barrier as the A chunk.
+// * Two consumer warpgroups (M = 64 rows each, N = BN, K = 8 per instruction) read their A fragments from the swizzled
+//   stage with conflict-free 32-bit shared loads, split them into (hi, lo) in registers and issue the register-A (RS)
+//   form of wgmma against the B images in shared memory.
 // * Epilogue: each consumer thread applies rowscale / BN / bias / residual / LeakyReLU to its accumulator registers
 //   and stores them straight to global memory.
+// * Footprint: 9 warps; for BN <= 64 a CTA stays within half an SM's registers and shared memory, so two GEMM CTAs,
+//   or one GEMM CTA and the kernels of another stream, share an SM and cover each other's k-chunk drains and epilogues.
+#include <cuda.h>
+#include <cudaTypedefs.h>
 #include <stdlib.h>
 
 #include "ops.cuh"
@@ -21,9 +26,8 @@ namespace d3f {
 
 constexpr int kTcBM = 128;       // rows per tile (two wgmma warpgroups of M = 64)
 constexpr int kTcBK = 32;        // fp32 per k-chunk = one 128 B swizzle row
-constexpr int kTcProducerThreads = 128;
 constexpr int kTcConsumerWarps = 8;
-constexpr int kTcThreads = kTcProducerThreads + 32 * kTcConsumerWarps;  // 1 producer + 2 consumer warpgroups
+constexpr int kTcThreads = 32 * kTcConsumerWarps + 32;   // 2 consumer warpgroups (warps 0-7) + 1 producer warp
 
 // ---------------------------------------------------------------------------------------------------
 // W[K,N] row-major -> packed[Kpad/32][2][Npad][32]: for every 32-wide k-chunk a (hi, lo) pair of ready-made shared
@@ -65,43 +69,53 @@ int tc_pack_weight(const float* W, int K, int N, float* packed, cudaStream_t str
 // Accumulation. Each k-chunk (12 wgmmas) is summed into a fresh register fragment that the consumer adds to the running
 // sum with round-to-nearest once the chunk has retired: the tensor pipe's own fp32 accumulate is biased towards zero,
 // and restarting it every chunk keeps that chain 12 MMAs long whatever K is. Measured on an H100 SXM (400 W power
-// limit) against one running accumulator with the next chunk's wgmmas overlapping the previous chunk's (wait_group 1),
-// M x K x N = 4096 x 7680 x 512, max-norm error vs float64: 1.2e-6 vs 8.5e-5 on all-positive data (mean signed error
-// -2.7e-7 vs -7.9e-5), 8.4e-7 vs 6.0e-5 on normal data; time 0.354 vs 0.393 ms (60000 x 960 x 64: 0.154 vs 0.156 ms),
-// so the wait after each chunk does not cost time at these shapes.
+// limit) against one running accumulator, M x K x N = 4096 x 7680 x 512, max-norm error vs float64: 1.2e-6 vs 8.5e-5
+// on all-positive data (mean signed error -2.7e-7 vs -7.9e-5), 8.4e-7 vs 6.0e-5 on normal data.
 //
-// Ring depth: the deepest ring of whole stages that fits the 227 KB of an H100 SM (one CTA of 12 warps per SM).
+// Inside a chunk each K = 8 step is one commit group and two steps are in flight (wait_group 1), so only two steps'
+// split A fragments are live. A consumer does wait for the chunk's last step before the next chunk: overlapping two
+// chunks would keep two accumulators live, which rules out two CTAs per SM; the other warpgroup and the second CTA keep
+// the tensor pipe busy across that drain instead.
+//
+// Ring: a stage is one raw A chunk (16 KB) + the B hi/lo images. BN <= 64: two CTAs per SM, so <= 96 registers per
+// thread (9 warps per CTA: one of the SM's four register-file quarters holds 5 of the 18 warps) and <= 113 KB of shared
+// memory each; BN = 128 (64-register accumulators) keeps one CTA per SM and 3 stages.
 template <int BN>
 struct TcSmem {
-  static constexpr int kStages = BN >= 128 ? 3 : 4;
-  static constexpr int kABytes = kTcBM * 128;  // one image (hi or lo) of the A tile
-  static constexpr int kBBytes = BN * 128;
-  static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;
+  static constexpr int kCtasPerSm = BN >= 128 ? 1 : 2;
+  static constexpr int kStages = BN >= 64 ? 3 : 4;
+  static constexpr int kABytes = kTcBM * 128;  // the raw fp32 A tile of one k-chunk
+  static constexpr int kBBytes = BN * 128;     // one image (hi or lo) of the B tile
+  static constexpr int kStageBytes = kABytes + 2 * kBBytes;
   static constexpr int kTotal = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/;
-  static_assert(kTotal <= 232448, "shared memory budget of an H100 SM (227 KB)");
+  static_assert(kCtasPerSm * (kTotal + 1024) <= 233472, "shared memory of an H100 SM (228 KB, 1 KB reserved per CTA)");
 };
 
 // One kernel for both launch shapes: grid.x = every output tile (one tile per CTA; split-K over grid.z) or fewer CTAs
-// than tiles (persistent: CTA b takes tiles b, b + gridDim.x, ...; the producers' ring runs across tile boundaries, so
+// than tiles (persistent: CTA b takes tiles b, b + gridDim.x, ...; the producer's ring runs across tile boundaries, so
 // the next tile's operands load while the consumers run the epilogue of the current one). n-tiles of one row block are
 // neighbours in the tile order: the A rows stay in L2.
+//
+// tmA / tmA2: tensor maps of the A operand, [A | A2] along K when K1 < Kpad (K1 = columns of A, a multiple of the
+// k-chunk, so a whole k-chunk comes from one of the two matrices). Rows past the device row count ep.m_dev but below the
+// capacity are loaded but never stored.
 template <int BN>
-__global__ void __launch_bounds__(kTcThreads, 1)
-tc_gemm_kernel(const float* __restrict__ A, const float* __restrict__ A2, int K1, const float* __restrict__ Bp,
-               float* __restrict__ C, int Mcap, int N, int K, int Kpad, int Npad, int chunks_per_split, Epilogue ep) {
+__global__ void __launch_bounds__(kTcThreads, TcSmem<BN>::kCtasPerSm)
+tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2, int K1,
+               const float* __restrict__ Bp, float* __restrict__ C, int Mcap, int N, int Kpad, int Npad,
+               int chunks_per_split, Epilogue ep) {
   // the split-K slabs are laid out with the launch capacity; the rows that exist come from device memory if given
   const int M = ep.m_dev ? min(Mcap, max(__ldg(ep.m_dev) - ep.m_off, 0)) : Mcap;
   const int ntn = Npad / BN;
   const int tiles = ceil_div(M, kTcBM) * ntn;
   if ((int)blockIdx.x >= tiles) return;   // CTA-uniform, before any barrier
-  const int my_tiles = (tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
   extern __shared__ uint8_t smem_raw[];
   using S = TcSmem<BN>;
   constexpr int kStages = S::kStages;
   // 1024 B alignment: SWIZZLE_128B atoms are 8 rows x 128 B and the swizzle uses absolute address bits
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* full = (uint64_t*)(smem + kStages * S::kStageBytes);   // [kStages] split A images + B images landed
-  uint64_t* empty = full + kStages;                                // [kStages] the wgmmas that read the stage retired
+  uint64_t* full = (uint64_t*)(smem + kStages * S::kStageBytes);   // [kStages] A chunk + B images landed
+  uint64_t* empty = full + kStages;                                // [kStages] the consumers are done with the stage
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   // split-K: CTA z owns the k-chunks [kt0, kt0 + nk) and writes raw partial sums to its own [M,N] slab of C
@@ -111,133 +125,99 @@ tc_gemm_kernel(const float* __restrict__ A, const float* __restrict__ A2, int K1
 
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) {
-      mbar_init(smem_u32(&full[s]), kTcProducerThreads + 1);   // + the TMA issuer's arrive.expect_tx
+      mbar_init(smem_u32(&full[s]), 1);                        // the producer's arrive.expect_tx
       mbar_init(smem_u32(&empty[s]), kTcConsumerWarps);        // one arrive per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
-  if (warp < 4) {
-    // ===================== producers: global --cp.async--> swizzled stage --(in-place hi/lo split)--> wgmma =====
-    // Every thread owns fixed 16-byte pieces of the stage (row = it*16 + rsub, chunk = tid & 7). It copies them
-    // asynchronously kStages-1 k-chunks ahead (A raw fp32 into the "hi" image, pre-split B into both images by TMA;
-    // rows beyond M / K are zero-filled), and when ITS OWN copy group of chunk g has landed (cp.async.wait_group is
-    // per thread, so no extra barrier) it splits its A pieces in place: hi overwrites the raw value, lo goes to the
-    // second image.
-    const int chunk = tid & 7;      // 16-byte chunk inside the 128-byte row
-    const int rsub = tid >> 3;      // 0..15: row inside a 16-row slab
-    const int total = my_tiles * nk;
-    int i_tile = (int)blockIdx.x, i_kt = 0, i_g = 0;         // the next chunk to copy: (tile, k-chunk), running number
-    auto issue_chunk = [&]() {
-      const int s = i_g % kStages;
-      mbar_wait(smem_u32(&empty[s]), ((uint32_t)(i_g / kStages) & 1u) ^ 1u);   // stage free (its wgmmas retired)
-      uint8_t* st = smem + s * S::kStageBytes;
-      const int m0 = (i_tile / ntn) * kTcBM, n0 = (i_tile % ntn) * BN;
-      // the A operand is [A | A2] along K when A2 is given (K1 = columns of A, a multiple of the k-chunk): a whole
-      // k-chunk comes from one of the two row-major matrices
-      int k0 = (kt0 + i_kt) * kTcBK + chunk * 4;
-      const float* src = A;
-      int ld = K;
-      if (A2 != nullptr) {
-        ld = K1;
-        if (k0 >= K1) {
-          src = A2;
-          ld = K - K1;
-          k0 -= K1;
+  if (warp == kTcConsumerWarps) {
+    // ===================== producer: one thread issues every copy of the ring ==============================
+    if (lane == 0) {
+      const int total = (tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x * nk;   // chunks of my tiles
+      int tile = (int)blockIdx.x, kt = 0;
+      for (int g = 0; g < total; ++g) {
+        const int s = g % kStages;
+        mbar_wait(smem_u32(&empty[s]), ((uint32_t)(g / kStages) & 1u) ^ 1u);   // stage free
+        const uint32_t st = smem_u32(smem + s * S::kStageBytes);
+        const uint32_t fb = smem_u32(&full[s]);
+        const int m0 = (tile / ntn) * kTcBM, n0 = (tile % ntn) * BN;
+        const int k0 = (kt0 + kt) * kTcBK;
+        mbar_arrive_expect_tx(fb, (uint32_t)S::kStageBytes);
+        if (k0 < K1)
+          tma_load_2d(st, &tmA, k0, m0, fb);
+        else
+          tma_load_2d(st, &tmA2, k0 - K1, m0, fb);
+        // B operand of this k-chunk: two contiguous pre-swizzled images (hi, lo) of BN rows x 128 B
+        const float* slab = Bp + (size_t)(kt0 + kt) * 2 * Npad * 32 + (size_t)n0 * 32;
+        tma_bulk_g2s(st + S::kABytes, slab, S::kBBytes, fb);
+        tma_bulk_g2s(st + S::kABytes + S::kBBytes, slab + (size_t)Npad * 32, S::kBBytes, fb);
+        if (++kt == nk) {
+          kt = 0;
+          tile += (int)gridDim.x;
         }
       }
-#pragma unroll
-      for (int it = 0; it < kTcBM / 16; ++it) {
-        const int row = it * 16 + rsub;
-        const int gm = m0 + row;
-        const uint32_t off = (uint32_t)row * 128u + (uint32_t)((chunk ^ (row & 7)) << 4);
-        const bool ok = gm < M && k0 < ld;
-        cp_async16_zfill(smem_u32(st + off), src + (size_t)(ok ? gm : 0) * ld + (ok ? k0 : 0), ok);
-      }
-      if (tid == 0) {
-        // B operand of this k-chunk: two contiguous pre-swizzled images (hi, lo) of BN rows x 128 B -> two TMA bulk
-        // copies that complete on the stage's "full" barrier
-        const uint32_t fb = smem_u32(&full[s]);
-        const float* slab = Bp + (size_t)(kt0 + i_kt) * 2 * Npad * 32 + (size_t)n0 * 32;
-        mbar_arrive_expect_tx(fb, 2u * S::kBBytes);
-        tma_bulk_g2s(smem_u32(st + 2 * S::kABytes), slab, S::kBBytes, fb);
-        tma_bulk_g2s(smem_u32(st + 2 * S::kABytes + S::kBBytes), slab + (size_t)Npad * 32, S::kBBytes, fb);
-      }
-      ++i_g;
-      if (++i_kt == nk) {
-        i_kt = 0;
-        i_tile += (int)gridDim.x;
-      }
-    };
-    for (int i = 0; i < kStages - 1; ++i) {
-      if (i < total) issue_chunk();
-      asm volatile("cp.async.commit_group;" ::: "memory");
-    }
-    for (int g = 0; g < total; ++g) {
-      const int s = g % kStages;
-      asm volatile("cp.async.wait_group %0;" ::"n"(kStages - 2) : "memory");   // this thread's pieces of chunk g landed
-      // all of this thread's pieces are read before anything is written back: the loads are independent of the
-      // in-place stores (which the compiler could not prove), so the eight shared-memory round trips overlap
-      const uint32_t st_s = smem_u32(smem + s * S::kStageBytes);
-      float4 x[kTcBM / 16];
-#pragma unroll
-      for (int it = 0; it < kTcBM / 16; ++it) {
-        const int row = it * 16 + rsub;
-        x[it] = lds128(st_s + (uint32_t)row * 128u + (uint32_t)((chunk ^ (row & 7)) << 4));
-      }
-#pragma unroll
-      for (int it = 0; it < kTcBM / 16; ++it) {
-        const int row = it * 16 + rsub;
-        const uint32_t off = (uint32_t)row * 128u + (uint32_t)((chunk ^ (row & 7)) << 4);
-        float4 hi, lo;
-        split_tf32(x[it].x, hi.x, lo.x);
-        split_tf32(x[it].y, hi.y, lo.y);
-        split_tf32(x[it].z, hi.z, lo.z);
-        split_tf32(x[it].w, hi.w, lo.w);
-        sts128(st_s + off, hi);
-        sts128(st_s + S::kABytes + off, lo);
-      }
-      fence_proxy_async();   // generic-proxy writes -> visible to the tensor core (async proxy)
-      mbar_arrive(smem_u32(&full[s]));
-      if (i_g < total) issue_chunk();
-      asm volatile("cp.async.commit_group;" ::: "memory");        // possibly empty: keeps the group count uniform
     }
   } else {
     // ===================== consumers: two warpgroups, 64 rows of the tile each ==============================
     // Per k-chunk and K = 8 step three wgmmas (3xTF32): Ah.Bh + Al.Bh + Ah.Bl (the Al.Bl term, ~2^-22 relative, is
     // dropped). Then the stage is released and the chunk's fragment joins the running sum.
     constexpr int R = BN / 2;                 // accumulator registers per thread (m64 x BN per warpgroup)
-    const int cw = (warp - 4) >> 2;           // consumer warpgroup: tile rows [64 cw, 64 cw + 64)
+    const int cw = warp >> 2;                 // consumer warpgroup: tile rows [64 cw, 64 cw + 64)
     const int wq = warp & 3;                  // warp inside the warpgroup: rows 16 wq .. 16 wq + 15 of its 64
+    // this thread's A fragment: rows r0 and r0 + 8, columns 8 j + t and 8 j + t + 4 of every K = 8 step j. In the
+    // SWIZZLE_128B stage row r holds its 16-byte pieces XOR-ed with r % 8 (the same for r0 and r0 + 8): the eight
+    // rows of a warp's load hit eight different pieces, the four threads of a row four banks of one piece.
+    const int r0 = 64 * cw + 16 * wq + (lane >> 2);
+    const uint32_t a_row = (uint32_t)r0 * 128u + (uint32_t)(lane & 3) * 4u, a_swz = (uint32_t)(r0 & 7);
+    // x[q] = A[r0 + 8 (q & 1)][8 j + t + 4 (q >> 1)] of the stage at sa: the tf32 fragment order of wgmma_tf32_rs
+    auto load_a = [&](float* x, uint32_t sa, int j) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        x[q] = lds32(sa + a_row + (uint32_t)(q & 1) * 1024u + ((((uint32_t)(2 * j + (q >> 1))) ^ a_swz) << 4));
+    };
     const bool has_bn = ep.bn_scale != nullptr, has_bias = ep.bias != nullptr, has_res = ep.residual != nullptr;
     const bool has_leaky = ep.leaky_alpha >= 0.f;
     const bool pairs = (N & 1) == 0;          // two adjacent columns of a row are one aligned 8-byte access
     float acc[R], sum[R];
     int g = 0;
-    for (int i = 0; i < my_tiles; ++i) {
-      const int t = (int)blockIdx.x + i * (int)gridDim.x;
+    for (int t = (int)blockIdx.x; t < tiles; t += (int)gridDim.x) {
       const int m0 = (t / ntn) * kTcBM, n0 = (t % ntn) * BN;
 #pragma unroll
       for (int j = 0; j < R; ++j) sum[j] = 0.f;
       for (int kt = 0; kt < nk; ++kt, ++g) {
         const int s = g % kStages;
         mbar_wait(smem_u32(&full[s]), (uint32_t)(g / kStages) & 1u);
+        const uint32_t sa = smem_u32(smem + s * S::kStageBytes);
+        const uint64_t b_hi = make_smem_desc(sa + S::kABytes), b_lo = make_smem_desc(sa + S::kABytes + S::kBBytes);
+        // one commit group per K = 8 step; the split fragment of step j lives in buffer j % 2 until wait_group 1
+        // after step j + 1 has retired it, so at most two steps' fragments (16 registers) are live
+        float x[4];
+        uint32_t ah[2][4], al[2][4];
+        load_a(x, sa, 0);
 #pragma unroll
         for (int j = 0; j < R; ++j) acc[j] = 0.f;
-        wgmma_fence();
-        const uint32_t sa = smem_u32(smem + s * S::kStageBytes);
-        const uint64_t a_hi = make_smem_desc(sa + (uint32_t)cw * (64 * 128));
-        const uint64_t a_lo = make_smem_desc(sa + S::kABytes + (uint32_t)cw * (64 * 128));
-        const uint64_t b_hi = make_smem_desc(sa + 2 * S::kABytes), b_lo = make_smem_desc(sa + 2 * S::kABytes + S::kBBytes);
 #pragma unroll
         for (int j = 0; j < kTcBK / 8; ++j) {
+          uint32_t* h = ah[j & 1];
+          uint32_t* l = al[j & 1];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            float hi, lo;
+            split_tf32(x[q], hi, lo);
+            h[q] = __float_as_uint(hi);
+            l[q] = __float_as_uint(lo);
+          }
           const uint64_t adv = (uint64_t)((j * 32) >> 4);   // +32 B per K = 8 step inside the swizzle atom
-          wgmma_tf32<BN>(acc, a_hi + adv, b_hi + adv);
-          wgmma_tf32<BN>(acc, a_lo + adv, b_hi + adv);
-          wgmma_tf32<BN>(acc, a_hi + adv, b_lo + adv);
+          wgmma_fence();
+          wgmma_tf32_rs<BN>(acc, h, b_hi + adv);
+          wgmma_tf32_rs<BN>(acc, l, b_hi + adv);
+          wgmma_tf32_rs<BN>(acc, h, b_lo + adv);
+          wgmma_commit();
+          if (j + 1 < kTcBK / 8) load_a(x, sa, j + 1);
+          wgmma_wait<1>();
         }
-        wgmma_commit();
         wgmma_wait<0>();
         wgmma_reg_fence<R>(acc);
         __syncwarp();
@@ -245,7 +225,6 @@ tc_gemm_kernel(const float* __restrict__ A, const float* __restrict__ A2, int K1
 #pragma unroll
         for (int j = 0; j < R; ++j) sum[j] += acc[j];
       }
-
       // ===================== epilogue straight from the registers ===========================================
       // A thread holds two rows (l/4 and l/4 + 8 of its warp's 16) x pairs of adjacent columns: the four lanes of a
       // row cover 8 consecutive columns, i.e. every 32-byte sector a warp stores or loads (residual) is whole.
@@ -316,7 +295,31 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restr
   }
 }
 
-// persistent = true: at most one CTA per SM, each walking several tiles (see tc_gemm_kernel)
+// 2D tensor map of a row-major fp32 matrix [rows, cols] (cols % 4 == 0, 16-byte aligned): boxes of 128 rows x one
+// k-chunk, SWIZZLE_128B (the K-major layout the consumers' fragment loads expect), zero fill out of bounds. The driver's
+// encoder is looked up through the runtime, so the library does not need libcuda to load (the CPU-only build imports it).
+static int encode_a_map(CUtensorMap* map, const float* A, int rows, int cols) {
+  static PFN_cuTensorMapEncodeTiled_v12000 encode = nullptr;
+  if (encode == nullptr) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    D3F_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q));
+    D3F_REQUIRE(q == cudaDriverEntryPointSuccess && fn != nullptr, D3F_ERR_CUDA,
+                "tc_gemm: the driver has no cuTensorMapEncodeTiled");
+    encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
+  }
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)cols * sizeof(float)};
+  const cuuint32_t box[2] = {(cuuint32_t)kTcBK, (cuuint32_t)kTcBM};
+  const cuuint32_t elem[2] = {1, 1};
+  const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(A), dims, strides, box, elem,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  D3F_REQUIRE(r == CUDA_SUCCESS, D3F_ERR_CUDA, "tc_gemm: cuTensorMapEncodeTiled failed (%d)", (int)r);
+  return D3F_OK;
+}
+
+// persistent = true: at most kCtasPerSm CTAs per SM, each walking several tiles (see tc_gemm_kernel)
 template <int BN>
 static int launch_tc(const float* A, const float* A2, int K1, const float* Bp, float* C, int M, int N, int K,
                      const Epilogue& ep, cudaStream_t stream, int splits, float* split_ws, bool persistent) {
@@ -329,9 +332,22 @@ static int launch_tc(const float* A, const float* A2, int K1, const float* Bp, f
   const int Kpad = tc_padded_k(K), Npad = tc_padded_n(N);
   const int nk = Kpad / kTcBK;
   const int tiles = ceil_div(M, kTcBM) * (Npad / BN);
+  // the maps are kernel parameters: a CUDA graph capture records them by value
+  CUtensorMap tmA, tmA2;
+  if (A2 != nullptr) {
+    int rc = encode_a_map(&tmA, A, M, K1);
+    if (rc == D3F_OK) rc = encode_a_map(&tmA2, A2, M, K - K1);
+    if (rc != D3F_OK) return rc;
+  } else {
+    const int rc = encode_a_map(&tmA, A, M, K);
+    if (rc != D3F_OK) return rc;
+    tmA2 = tmA;
+    K1 = Kpad;
+  }
   if (splits <= 1) {
-    const int grid = persistent && tiles > kNumSMs ? kNumSMs : tiles;
-    tc_gemm_kernel<BN><<<grid, kTcThreads, S::kTotal, stream>>>(A, A2, K1, Bp, C, M, N, K, Kpad, Npad, nk, ep);
+    const int cap = kNumSMs * S::kCtasPerSm;
+    const int grid = persistent && tiles > cap ? cap : tiles;
+    tc_gemm_kernel<BN><<<grid, kTcThreads, S::kTotal, stream>>>(tmA, tmA2, K1, Bp, C, M, N, Kpad, Npad, nk, ep);
     D3F_LAUNCH_CHECK("tc_gemm_kernel");
     return D3F_OK;
   }
@@ -341,7 +357,7 @@ static int launch_tc(const float* A, const float* A2, int K1, const float* Bp, f
   raw.rowscale = nullptr; raw.bn_scale = nullptr; raw.bn_shift = nullptr; raw.bias = nullptr; raw.residual = nullptr;
   raw.leaky_alpha = -1.f; raw.row_map = nullptr; raw.m_dev = ep.m_dev; raw.m_off = ep.m_off;
   dim3 grid(tiles, 1, splits);
-  tc_gemm_kernel<BN><<<grid, kTcThreads, S::kTotal, stream>>>(A, A2, K1, Bp, split_ws, M, N, K, Kpad, Npad, cps, raw);
+  tc_gemm_kernel<BN><<<grid, kTcThreads, S::kTotal, stream>>>(tmA, tmA2, K1, Bp, split_ws, M, N, Kpad, Npad, cps, raw);
   D3F_LAUNCH_CHECK("tc_gemm_kernel");
   long long total = (long long)M * N;
   int blocks = (int)min((total + 255) / 256, (long long)kNumSMs * 8);
