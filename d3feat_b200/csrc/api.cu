@@ -229,4 +229,14 @@ int d3f_affine_leaky(const float* x, int N, int C, const float* scale, const flo
   return affine_leaky(x, N, C, scale, shift, residual, leaky_alpha, out, (cudaStream_t)stream, n_dev);
 }
 
+size_t d3f_select_keypoints_workspace_bytes(int N, int B) { return select_keypoints_workspace_bytes(N, B); }
+
+int d3f_select_keypoints(const float* scores, const int* lengths, int B, int N, int k, const float* points,
+                         const float* descriptors, int D, int* out_order, int* out_index, int* out_count,
+                         float* out_points, float* out_descriptors, float* out_scores, void* workspace,
+                         size_t workspace_bytes, d3f_stream_t stream, const int* n_dev) {
+  return select_keypoints(scores, lengths, B, N, k, points, descriptors, D, out_order, out_index, out_count, out_points,
+                          out_descriptors, out_scores, workspace, workspace_bytes, (cudaStream_t)stream, n_dev);
+}
+
 }  // extern "C"

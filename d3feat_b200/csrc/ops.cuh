@@ -94,4 +94,11 @@ int detection_scores(const float* feats, const int* neighbors, const int* length
 int affine_leaky(const float* x, int N, int C, const float* scale, const float* shift, const float* residual,
                  float alpha, float* out, cudaStream_t stream, const int* n_dev = nullptr);
 
+// ---- keypoints.cu -----------------------------------------------------------------------------------
+size_t select_keypoints_workspace_bytes(int N, int B);
+int select_keypoints(const float* scores, const int* lengths, int B, int N, int k, const float* points,
+                     const float* descriptors, int D, int* out_order, int* out_index, int* out_count, float* out_points,
+                     float* out_descriptors, float* out_scores, void* workspace, size_t workspace_bytes,
+                     cudaStream_t stream, const int* n_dev = nullptr);
+
 }  // namespace d3f

@@ -7,12 +7,18 @@ executes the tf.data pyramid on the CPU and the network on the device); here bot
     enc = KPFCNN(config, params, neighborhood_limits)
     out = enc(points_host_or_cuda, lengths)           # pyramid + encoder (+ decoder)
 """
+from collections import namedtuple
+
 import numpy as np
 import torch
 
 from . import network_blocks as nb
 from . import pyramid
+from .keypoints import select_keypoints
 from .variables import ParamStore, use_params
+
+# GraphPipeline(..., keypoints=k) result: descriptors [cap0,32], scores [cap0,1], keypoints (KeypointSet, k per cloud)
+Detections = namedtuple("Detections", "descriptors scores keypoints")
 
 
 class KPFCNN:
@@ -60,12 +66,20 @@ class KPFCNN:
         with use_params(self.store):
             return nb.assemble_FCNN_decoder(inputs, self.config, F, 1.0, with_scores=with_scores)
 
-    def __call__(self, stacked_points, stacked_lengths, features=None, bbox=None, decoder=None):
+    def __call__(self, stacked_points, stacked_lengths, features=None, bbox=None, decoder=None, num_keypoints=None):
+        """num_keypoints=k (decoder runs): the result also holds "keypoints", the KeypointSet of the k highest-scoring
+        level-0 points of every cloud (keypoints.select_keypoints)."""
         inputs = self.build_inputs(stacked_points, stacked_lengths, features, bbox)
         F = self.encode(inputs)
         use_dec = self.has_decoder if decoder is None else decoder
+        if num_keypoints is not None and not use_dec:
+            raise ValueError("KPFCNN: num_keypoints needs the decoder (its detection scores)")
         desc, scores = self.describe(inputs, F, with_scores=True) if use_dec else (None, None)
-        return dict(inputs=inputs, F=F, descriptors=desc, scores=scores)
+        out = dict(inputs=inputs, F=F, descriptors=desc, scores=scores)
+        if num_keypoints is not None:
+            out["keypoints"] = select_keypoints(scores, inputs["lengths"][0], num_keypoints,
+                                                points=inputs["points"][0], descriptors=desc)
+        return out
 
 
 class BatchPipeline:
@@ -191,11 +205,20 @@ class GraphPipeline:
 
     `res` is the slot's static output buffer [capacity of the last level, C] and `counts` the device int32 level sizes
     (counts[l] for level l < L; rows of `res` beyond counts[L - 1] are undefined); both stay valid until the slot is
-    reused DEPTH steps later. Mirrors the overlap the reference gets from tf.data prefetch (datasets/common.py:744-763)."""
+    reused DEPTH steps later. Mirrors the overlap the reference gets from tf.data prefetch (datasets/common.py:744-763).
+
+    keypoints=k (needs decoder=True): the encoder graph also runs the detection scores and the per-cloud top-k
+    selection, and `res` is a Detections(descriptors [cap0,32], scores [cap0,1], keypoints) whose KeypointSet holds
+    the k highest-scoring level-0 points of every cloud -- slot buffers too, valid for the same DEPTH steps."""
 
     DEPTH = 4
 
-    def __init__(self, enc, capacities, n_clouds, bbox, decoder=False, post=None, encoder_streams=2):
+    def __init__(self, enc, capacities, n_clouds, bbox, decoder=False, post=None, encoder_streams=2, keypoints=None):
+        if keypoints is not None and not decoder:
+            raise ValueError("GraphPipeline: keypoints=%r needs decoder=True (the detection scores)" % (keypoints,))
+        if keypoints is not None and int(keypoints) < 1:
+            raise ValueError("GraphPipeline: keypoints=%r must be >= 1" % (keypoints,))
+        self.keypoints = None if keypoints is None else int(keypoints)
         self.enc, self.decoder, self.post = enc, decoder, post
         dev = enc.device
         self.caps = [int(c) for c in capacities]
@@ -238,6 +261,11 @@ class GraphPipeline:
 
     def _run_encoder(self, inputs):
         F = self.enc.encode(inputs)
+        if self.keypoints is not None:
+            desc, scores = self.enc.describe(inputs, F, with_scores=True)
+            kp = select_keypoints(scores, inputs["lengths"][0], self.keypoints, points=inputs["points"][0],
+                                  descriptors=desc, rows=inputs["rows"][0])
+            return F, Detections(desc, scores, kp)
         res = self.enc.describe(inputs, F) if self.decoder else F[-1]
         return F, res
 

@@ -1,0 +1,69 @@
+"""Keypoint detection on the GPU: per-cloud selection by detection score (d3f_select_keypoints).
+
+The reference selects keypoints on the host after every batch: the 3DMatch tester dumps each fragment's points,
+descriptors and scores sorted by score and the evaluation keeps the last 250 rows (utils/tester.py:209-213,
+geometric_registration/evaluate.py:45-50); the KITTI tester keeps the top 250 per cloud (utils/tester.py:281-290).
+Here all clouds of a stack are ordered by one device sort, with no host round trip, so the selection can run inside
+a captured CUDA graph (encoder.GraphPipeline(..., keypoints=k)).
+
+Order: within each cloud, ascending score, ties by ascending row -- np.argsort(s_b, kind="stable") -- with every NaN
+(either sign) above +inf and -0.0 equal to +0.0. The top k of cloud b are argsort(s_b, kind="stable")[-k:] + start_b.
+This is deliberately not io_utils.select_keypoints' order: that function uses numpy's default argsort, whose tie order
+depends on the numpy build; on tie-free scores the two agree.
+"""
+from collections import namedtuple
+
+import torch
+
+from . import _lib
+
+KeypointSet = namedtuple("KeypointSet", "index count points descriptors scores")
+KeypointSet.__doc__ = """Fixed-shape keypoints of B clouds, k slots each (slots j >= count[b] hold index -1 and zeros).
+    index [B,k] int32 global rows, count [B] int32 = min(k, len_b), points [B,k,3], descriptors [B,k,D] and scores
+    [B,k] float32 (None when the matching input was not given). Slots are in ascending score order."""
+
+
+def select_keypoints(scores, lengths, k=None, points=None, descriptors=None, *, rows=None):
+    """scores [N] or [N,1] (CUDA float32), lengths [B] stack lengths.
+
+    k=None: the full order int32 [N] -- every row, clouds in stack order, ascending score within each (the 3DMatch
+    tester's layout). k: a KeypointSet with the top min(k, len_b) rows of every cloud, gathered from `points` [N,3]
+    and `descriptors` [N,D] when given.
+    rows: optional device int32 scalar with the actual row count (the static pyramid's level-0 count); N is then the
+    capacity of the inputs and no row at or past it is read (order[rows:] is left unwritten)."""
+    s = scores.reshape(-1)
+    if not s.is_cuda or s.dtype != torch.float32:
+        raise ValueError("select_keypoints: scores must be a CUDA float32 tensor")
+    s = s.contiguous()
+    dev = s.device
+    lens = _lib.i32(lengths, dev)
+    N, B = int(s.shape[0]), int(lens.shape[0])
+    pts = _lib.f32(points, dev) if points is not None else None
+    desc = _lib.f32(descriptors, dev) if descriptors is not None else None
+    if pts is not None and tuple(pts.shape) != (N, 3):
+        raise ValueError("select_keypoints: points %s do not match %d scores" % (tuple(pts.shape), N))
+    if desc is not None and (desc.dim() != 2 or int(desc.shape[0]) != N):
+        raise ValueError("select_keypoints: descriptors %s do not match %d scores" % (tuple(desc.shape), N))
+    D = int(desc.shape[1]) if desc is not None else 0
+    lib = _lib.lib()
+    ws = _lib.workspace(lib.d3f_select_keypoints_workspace_bytes(N, B), dev)
+    i32, f32 = torch.int32, torch.float32
+    if k is None:
+        order = torch.empty((N,), dtype=i32, device=dev)
+        _lib.check(lib.d3f_select_keypoints(_lib.ptr(s), _lib.ptr(lens), B, N, 0, None, None, 0, _lib.ptr(order),
+                                            None, None, None, None, None, _lib.ptr(ws), ws.numel(), _lib.stream(),
+                                            _lib.ptr(rows)), "d3f_select_keypoints")
+        return order
+    k = int(k)
+    if k < 1:
+        raise ValueError("select_keypoints: k=%d must be >= 1" % k)
+    index = torch.empty((B, k), dtype=i32, device=dev)
+    count = torch.empty((B,), dtype=i32, device=dev)
+    out_s = torch.empty((B, k), dtype=f32, device=dev)
+    out_p = torch.empty((B, k, 3), dtype=f32, device=dev) if pts is not None else None
+    out_d = torch.empty((B, k, D), dtype=f32, device=dev) if desc is not None else None
+    _lib.check(lib.d3f_select_keypoints(_lib.ptr(s), _lib.ptr(lens), B, N, k, _lib.ptr(pts), _lib.ptr(desc), D, None,
+                                        _lib.ptr(index), _lib.ptr(count), _lib.ptr(out_p), _lib.ptr(out_d),
+                                        _lib.ptr(out_s), _lib.ptr(ws), ws.numel(), _lib.stream(), _lib.ptr(rows)),
+               "d3f_select_keypoints")
+    return KeypointSet(index, count, out_p, out_d, out_s)

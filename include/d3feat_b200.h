@@ -25,6 +25,7 @@
  *   d3f_ind_max_pool          models/network_blocks.py:51-66
  *   d3f_closest_pool          models/network_blocks.py:69-83
  *   d3f_l2_normalize          models/D3Feat.py:65
+ *   d3f_select_keypoints      utils/tester.py:209-213, 281-290 (host argsort of the detection scores)
  */
 #ifndef D3FEAT_B200_H_
 #define D3FEAT_B200_H_
@@ -250,6 +251,25 @@ int d3f_detection_scores(const float* feats, const int* neighbors, const int* le
 int d3f_affine_leaky(const float* x, int N, int C, const float* scale, const float* shift,
                      const float* residual, float leaky_alpha, float* out, d3f_stream_t stream,
                      const int* n_dev);
+
+/* Keypoint selection by detection score for B stacked clouds (utils/tester.py:209-213, the 3DMatch tester: every
+ * point in ascending score order; :281-290, the KITTI tester: the top k per cloud, ascending).
+ *   scores[N] (N = capacity with n_dev), lengths[B] (device), optional points[N,3] and descriptors[N,D].
+ *   Order contract: within each cloud, ascending score with ties by ascending row -- np.argsort(kind="stable") --
+ *   where every NaN (either sign) ranks above +inf and -0.0 equals +0.0.
+ *   Outputs (each optional, at least one required):
+ *     out_order[N]       every row: clouds in stack order, ascending score within each (rows >= n untouched)
+ *     out_index[B,k]     global rows of cloud b's top min(k, len_b), ascending score (= argsort(s_b)[-k:] + start_b)
+ *     out_count[B]       min(k, len_b)
+ *     out_points[B,k,3], out_descriptors[B,k,D], out_scores[B,k]   the selected rows
+ *   Slots j >= count_b hold index -1 and zero rows. A cloud reaching past n (lengths summing to more than n) is cut at
+ *   n: no row >= n is read. Rows past the last cloud (lengths summing to less than n) belong to no cloud and come
+ *   last in out_order. k >= 1 when a per-cloud output is requested; D >= 1 with descriptors. Graph-capturable. */
+size_t d3f_select_keypoints_workspace_bytes(int N, int B);
+int d3f_select_keypoints(const float* scores, const int* lengths, int B, int N, int k, const float* points,
+                         const float* descriptors, int D, int* out_order, int* out_index, int* out_count,
+                         float* out_points, float* out_descriptors, float* out_scores, void* workspace,
+                         size_t workspace_bytes, d3f_stream_t stream, const int* n_dev);
 
 #ifdef __cplusplus
 }
