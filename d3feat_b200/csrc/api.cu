@@ -217,7 +217,7 @@ size_t d3f_detection_scores_workspace_bytes(int N, int B) { return detection_sco
 int d3f_detection_scores(const float* feats, const int* neighbors, const int* lengths, int B, int N, int H, int D,
                          float* out_scores, void* workspace, size_t workspace_bytes, d3f_stream_t stream,
                          const int* n_dev) {
-  D3F_REQUIRE(N == 0 || (feats && neighbors && lengths && out_scores && workspace), D3F_ERR_INVALID,
+  D3F_REQUIRE(N == 0 || (feats && (neighbors || H == 0) && lengths && out_scores && workspace), D3F_ERR_INVALID,
               "d3f_detection_scores: null pointer");
   return detection_scores(feats, neighbors, lengths, B, N, H, D, out_scores, workspace, workspace_bytes,
                           (cudaStream_t)stream, n_dev);

@@ -172,7 +172,8 @@ int l2_normalize(const float* x, int N, int C, float eps, float* out, cudaStream
 // ---------------------------------------------------------------------------------------------------
 // Detection score of D3Feat (models/D3Feat.py:67-115), generalised from the reference's hard-coded pair of clouds to
 // B stacked clouds: per-cloud max normalisation, density-invariant saliency softplus(x - mean of the neighbours whose
-// feature-row sum is non-zero), channel-max ratio, max over channels.
+// feature-row sum is non-zero), channel-max ratio, max over channels. Rows at or past start[B] (lengths summing to less
+// than the row count) belong to no cloud: they take no part in any cloud's maximum, and their own score is unspecified.
 __global__ void __launch_bounds__(256)
 cloud_max_kernel(const float* __restrict__ x, int Ncap, const int* __restrict__ n_dev, int D,
                  const int* __restrict__ start, int B, unsigned* __restrict__ cloud_max_ord,
@@ -192,7 +193,7 @@ cloud_max_kernel(const float* __restrict__ x, int Ncap, const int* __restrict__ 
     s += __shfl_xor_sync(0xffffffffu, s, o);
   }
   if (lane == 0) {
-    atomicMax(&cloud_max_ord[batch_of(start, B, warp)], f2ord(m));
+    if (warp < start[B]) atomicMax(&cloud_max_ord[batch_of(start, B, warp)], f2ord(m));
     nonzero[warp] = s != 0.f ? 1 : 0;   // tf.count_nonzero of the neighbour's channel sum (:91-92)
   }
 }
@@ -205,8 +206,9 @@ detection_score_kernel(const float* __restrict__ x, const int* __restrict__ nb, 
   const int N = dyn_rows(Ncap, n_dev);
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= N) return;
-  // all neighbours of a point lie in its own cloud, so one scale serves the point and its neighbourhood
-  const float inv = 1.f / (ord2f(cloud_max_ord[batch_of(start, B, warp)]) + 1e-6f);
+  // all neighbours of a point lie in its own cloud, so one scale serves the point and its neighbourhood; a row of no
+  // cloud gets scale 0
+  const float inv = warp < start[B] ? 1.f / (ord2f(cloud_max_ord[batch_of(start, B, warp)]) + 1e-6f) : 0.f;
   const int* row = nb + (size_t)warp * H;
   int cnt = 0;
   for (int h = 0; h < H; ++h) {

@@ -239,7 +239,10 @@ int d3f_unary_pair_forward(const float* x1, int Cin1, const float* x2, int Cin2,
 
 /* Detection score of D3Feat (models/D3Feat.py:67-115) for B stacked clouds: feats[N,D] are the decoder outputs BEFORE
  * l2 normalisation, neighbors[N,H] the level-0 conv neighbours (shadow index = N), lengths[B] the stack lengths.
- * out_scores[N]. The reference hard-codes B = 2 (anchor || positive); the result is identical for B = 2. */
+ * out_scores[N]. The reference hard-codes B = 2 (anchor || positive); the result is identical for B = 2.
+ * A cloud reaching past the row count n (lengths summing to more than n) is cut there. Rows past the last cloud
+ * (lengths summing to less than n) belong to no cloud: they enter no cloud's maximum, so they change no real row's
+ * score, and their own score is unspecified. */
 size_t d3f_detection_scores_workspace_bytes(int N, int B);
 int d3f_detection_scores(const float* feats, const int* neighbors, const int* lengths, int B, int N,
                          int H, int D, float* out_scores, void* workspace, size_t workspace_bytes,

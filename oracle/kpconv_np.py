@@ -374,7 +374,7 @@ class EncoderOracle:
         return feats / norm
 
 
-def detection_scores(features, neighbors, lengths):
+def detection_scores(features, neighbors, lengths, magnitude=False, rows=None, chunk=4096):
     """Detection branch, models/D3Feat.py:67-115, for any number of stacked clouds (the reference writes it out for
     exactly two: first_pcd / second_pcd of in_batches).
 
@@ -384,26 +384,84 @@ def detection_scores(features, neighbors, lengths):
                mean = sum over neighbours / neighbour_num; local_max_score = softplus(features - mean)
       :96-97   depth_wise_max_score = features / (1e-6 + max over channels)
       :99-104  score = max over channels of the product; the shadow row is dropped.
+
+    A cloud reaching past the N rows is cut at N; rows past the last cloud belong to no cloud (scaled to zero, in no
+    cloud's maximum). rows= evaluates the score of those rows only (the cloud maxima still come from whole clouds).
+
+    magnitude=True returns (score, mag, alt), all [len(rows), 1]:
+      mag  the first-order rounding-error scale of the score on absolute values: the cloud scale 1/(M + 1e-6) carries
+           the cancellation factor k = (|M| + 1e-6) / |M + 1e-6| into every scaled feature (mag_f = k |f|); the
+           neighbour mean sum_h k |f_h| / cnt; softplus adds slope sigma(d) times the error of d plus its own rounding;
+           the channel ratio f / (1e-6 + dmax) the relative errors of both operands, its denominator with the
+           cancellation factor of 1e-6 + dmax; the max over channels is 1-Lipschitz (mag = max over channels). One
+           float32 underflow step (FLT_MIN) is added to the softplus and the score.
+      alt  the score with the count_nonzero vote flipped for every neighbour whose channel sum is within NN_SUM_ULPS
+           of zero, exact zero included (a kernel sums the raw row in its own order, the restatement the scaled row;
+           either may come out at exactly zero). Rows whose channels are all zero are not marked. mag covers both.
     """
     x = np.asarray(features)
     dt = x.dtype.type
     N, D = x.shape
     lengths = np.asarray(lengths, np.int64)
+    start = np.minimum(np.concatenate([[0], np.cumsum(lengths)]), N)
     scaled = np.zeros((N + 1, D), x.dtype)
-    s = 0
-    for n in lengths:
-        if n > 0:
-            scaled[s:s + n] = x[s:s + n] / (x[s:s + n].max() + dt(1e-6))
-        s += n
-    nb = np.asarray(neighbors, np.int64)
-    nf = scaled[nb]                                           # [N, H, D]; shadow index N -> zero row
-    num = np.maximum(np.count_nonzero(nf.sum(axis=-1), axis=-1), 1).astype(x.dtype)[:, None]
-    mean = nf.sum(axis=1) / num
-    d = scaled[:N] - mean
-    softplus = np.where(d > 20, d, np.log1p(np.exp(np.minimum(d, dt(20)))))
-    dmax = scaled[:N].max(axis=1, keepdims=True)
-    score = (softplus * (scaled[:N] / (dt(1e-6) + dmax))).max(axis=1, keepdims=True)
-    return score.astype(x.dtype)
+    kappa = np.ones((N + 1, 1))                              # cancellation factor of the row's cloud scale
+    with np.errstate(divide="ignore", invalid="ignore"):
+        for b in range(len(lengths)):
+            a, e = start[b], start[b + 1]
+            if e > a:
+                m = x[a:e].max()
+                scaled[a:e] = x[a:e] / (m + dt(1e-6))
+                kappa[a:e] = (abs(float(m)) + 1e-6) / abs(float(m) + 1e-6)
+    rows = np.arange(N) if rows is None else np.asarray(rows, np.int64)
+    nb_all = np.asarray(neighbors, np.int64)
+    out = np.zeros((rows.shape[0], 1), x.dtype)
+    if magnitude:
+        mag, alt = np.zeros((rows.shape[0], 1)), np.zeros((rows.shape[0], 1), x.dtype)
+    tiny = float(np.finfo(np.float32).tiny)
+    for a, b in _chunks(rows.shape[0], chunk):
+        r = rows[a:b]
+        nb = nb_all[r]
+        nf = scaled[nb]                                       # [n, H, D]; shadow index N -> zero row
+        f = scaled[r]
+        nsum = nf.sum(axis=-1)
+        vote = nsum != 0
+        dmax = f.max(axis=1, keepdims=True)
+        ratio = f / (dt(1e-6) + dmax)
+
+        def branch(vote):
+            num = np.maximum(np.count_nonzero(vote, axis=-1), 1).astype(x.dtype)[:, None]
+            mean = nf.sum(axis=1) / num
+            d = f - mean
+            softplus = np.where(d > 20, d, np.log1p(np.exp(np.minimum(d, dt(20)))))
+            return (softplus * ratio).max(axis=1, keepdims=True), num, d, softplus
+
+        score, num, d, softplus = branch(vote)
+        out[a:b] = score
+        if not magnitude:
+            continue
+        asum = np.abs(nf).sum(axis=-1)
+        amb = np.abs(nsum) < NN_SUM_ULPS * asum
+        score2, num2, d2, softplus2 = branch(vote ^ amb)
+        alt[a:b] = score2
+        k = kappa[r]
+        af = k * np.abs(f)
+        dmax64 = dmax.astype(np.float64)
+        e = 1e-6 + dmax64
+        ae = k * np.abs(dmax64) + 1e-6
+        with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+            aratio = (af + np.abs(ratio) * ae) / np.abs(e)
+            an = (kappa[nb] * np.abs(nf)).sum(axis=1)          # sum_h k |f_h|
+            m = None
+            for nm, dd, sp in ((num, d, softplus), (num2, d2, softplus2)):
+                sig = 0.5 * (1.0 + np.tanh(0.5 * np.float64(dd)))
+                asp = sig * (af + an / nm) + np.abs(sp) + tiny
+                mp = (asp * np.abs(ratio) + np.abs(sp) * aratio).max(axis=1, keepdims=True)
+                m = mp if m is None else np.maximum(m, mp)
+        mag[a:b] = m + tiny
+    if magnitude:
+        return out, mag, alt
+    return out
 
 
 # ----------------------------------------------------------------------------------------------------

@@ -1,6 +1,6 @@
-"""Test infrastructure: record every fused op the GPU encoder launches (inputs and output, device tensors) so that
-the numpy restatement can be evaluated on a SAMPLE OF ROWS of each op at sizes where the full float64 restatement is
-too slow (BASELINE configs[1]/[2]/[3] at their real sizes). Each op is independent per output row, so checking
+"""Test infrastructure: record every fused op the GPU encoder and decoder launch (KPConv, unary GEMMs, both pools, the
+detection scores; inputs and output, device tensors) so that the numpy restatement can be evaluated on a SAMPLE OF
+ROWS of each op at sizes where the full float64 restatement is too slow (BASELINE configs[1]/[2]/[3] at their real sizes). Each op is independent per output row, so checking
 sampled rows against the oracle on the op's real inputs is an oracle comparison, not a path-vs-path one.
 """
 import contextlib
@@ -23,7 +23,7 @@ def record_ops():
     from d3feat_b200 import network_blocks as nb
     tr = Trace()
     orig = dict(kp=co.KPConv_ops, kd=co.KPConv_deform_ops, un=co.unary_convolution, up=co.unary_pair_convolution,
-                mp=nb.ind_max_pool)
+                mp=nb.ind_max_pool, cp=nb.closest_pool, ds=nb.detection_scores)
 
     def kp(q, s, idx, f, Kp, W, extent, infl, mode, *, epilogue=None, bias=None, query_order=None, **rows):
         out = orig["kp"](q, s, idx, f, Kp, W, extent, infl, mode, epilogue=epilogue, bias=bias, query_order=query_order,
@@ -58,14 +58,26 @@ def record_ops():
                                rows_s=rows.get("rows_x")))
         return out
 
+    def cp(x, inds, **rows):
+        out = orig["cp"](x, inds, **rows)
+        tr.records.append(dict(op="closest_pool", x=x, inds=inds, out=out, rows_q=rows.get("rows_out"),
+                               rows_s=rows.get("rows_x")))
+        return out
+
+    def ds(features, neighbors, lengths, *, rows=None):
+        out = orig["ds"](features, neighbors, lengths, rows=rows)
+        tr.records.append(dict(op="detection_scores", features=features, neighbors=neighbors, lengths=lengths, out=out,
+                               rows_q=rows))
+        return out
+
     co.KPConv_ops, co.KPConv_deform_ops, co.unary_convolution, co.unary_pair_convolution = kp, kd, un, up
-    nb.ind_max_pool = mp
+    nb.ind_max_pool, nb.closest_pool, nb.detection_scores = mp, cp, ds
     try:
         yield tr
     finally:
         co.KPConv_ops, co.KPConv_deform_ops, co.unary_convolution, co.unary_pair_convolution = (
             orig["kp"], orig["kd"], orig["un"], orig["up"])
-        nb.ind_max_pool = orig["mp"]
+        nb.ind_max_pool, nb.closest_pool, nb.detection_scores = orig["mp"], orig["cp"], orig["ds"]
 
 
 def _np(t):
@@ -140,6 +152,17 @@ def check_sampled_rows(trace, n_rows, rng, rtol, min_kpconv=None, tol=_o.TOL, wh
             assert np.array_equal(out[rows], ref), "ind_max_pool rows differ (exact op)"
             report.append((r["op"], out.shape, 0.0, 0.0))
             continue
+        elif r["op"] == "closest_pool":
+            x = _np(r["x"])[:_count(r.get("rows_s"), r["x"].shape[0])]
+            ref = _ok.closest_pool(x, _np(r["inds"])[rows])
+            assert np.array_equal(out[rows], ref), "closest_pool rows differ (exact op)"
+            report.append((r["op"], out.shape, 0.0, 0.0))
+            continue
+        elif r["op"] == "detection_scores":
+            # features and neighbours cut to the device count: the shadow index is the count, as on the device
+            x, nbr = _np(r["features"])[:N].astype(np.float64), _np(r["neighbors"])[:N]
+            assert nbr.min(initial=0) >= 0 and nbr.max(initial=0) <= N, "detection_scores: index past the row count"
+            ref, mag, alt = _ok.detection_scores(x, nbr, _np(r["lengths"]), magnitude=True, rows=rows)
         else:
             raise AssertionError(r["op"])
         err = float(np.abs(out[rows].astype(np.float64) - ref).max()) / denom

@@ -17,6 +17,7 @@ import os
 import subprocess
 import sys
 import tempfile
+import time
 import zlib
 
 import numpy as np
@@ -45,7 +46,11 @@ def launched(fn):
     """(result of fn(), set of kernel names it launched), from torch.profiler's CUDA activity."""
     from torch.profiler import ProfilerActivity, profile
     names = set()
-    for attempt in range(2):     # CUPTI occasionally delivers an empty activity buffer; the ops are deterministic
+    # CUPTI occasionally delivers an empty activity buffer, at times for two sessions in a row; the ops are
+    # deterministic, so the capture is simply repeated after a short pause
+    for attempt in range(5):
+        if attempt:
+            time.sleep(0.1)
         torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             out = fn()

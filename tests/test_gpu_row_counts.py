@@ -275,26 +275,58 @@ def test_row_wise_epilogues_row_count(cuda, n):
     check_tail(out, m, "affine_leaky")
 
 
-@pytest.mark.parametrize("n", COUNTS)
-def test_detection_scores_row_count(cuda, n):
-    """Scores are O(1) (products of two ratios in [0, 1] and a softplus), so the bound is absolute: 1e-5."""
+SCORE_ROW_CASES = [(n, None) for n in COUNTS] + [(CAP // 2 + 3, e) for e in (0, 37, -37)]
+
+
+def _score_lengths(m, excess):
+    """Seven clouds (empty and one-point ones among them) whose lengths sum to m + excess."""
+    lens = np.array([0, 1, 40, 0, 35, 1, 0], np.int64)
+    lens[-1] = m + excess - lens.sum()
+    assert lens[-1] > 0
+    return lens.astype(np.int32)
+
+
+@pytest.mark.parametrize("n,excess", SCORE_ROW_CASES,
+                         ids=[str(n) if e is None else "B7_excess%+d" % e for n, e in SCORE_ROW_CASES])
+def test_detection_scores_row_count(cuda, n, excess):
+    """One cloud of exactly n rows, or (excess given) seven clouds whose lengths sum to n + excess: more than n cuts
+    the last cloud at n, less than n leaves rows past the last cloud that belong to no cloud. Those rows hold a huge
+    maximum: they must not change any real row's score (compared with the oracle, and bit for bit with the same clouds
+    at n = sum of the lengths); their own score is unspecified. Element by element against float64."""
     from d3feat_b200 import _lib
     D = Keep(cuda)
     L, m = _lib.lib(), max(n, 0)
-    rng = np.random.default_rng(n + 9)
+    rng = np.random.default_rng(n + 9 + (0 if excess is None else 1000 + excess))
     dim, H = 32, 12
     x = np.abs(rng.normal(size=(CAP, dim))).astype(np.float32)
+    x[rng.uniform(size=CAP) < 0.1] = 0.0
+    lengths = np.array([m], np.int32) if excess is None else _score_lengths(m, excess)
+    start = np.minimum(np.concatenate([[0], np.cumsum(lengths)]), m)
+    real = int(start[-1])                                          # rows that belong to a cloud
     nbr = np.full((CAP, H), m, np.int32)
-    if m:
-        nbr[:m] = rng.integers(0, m + 1, (m, H))
+    for b in range(len(lengths)):                                  # neighbours within the cloud, or the shadow m
+        a, e = start[b], start[b + 1]
+        if e > a:
+            blk = rng.integers(a, e + 1, (e - a, H)).astype(np.int32)
+            blk[blk == e] = m
+            nbr[a:e] = blk
+    x[real:m] = 1e6                                                # rows of no cloud: a huge maximum
     nbr = wrong_indices(nbr, m, rng)
-    lengths = np.array([m], np.int32)
-    ws = _lib.workspace(L.d3f_detection_scores_workspace_bytes(CAP, 1), cuda)
+    ws = _lib.workspace(L.d3f_detection_scores_workspace_bytes(CAP, len(lengths)), cuda)
     out = sentinel_out(CAP, 1, cuda)
-    call(L.d3f_detection_scores(D(poisoned(x, m)), D(nbr), D(lengths), 1, CAP, H, dim,
+    call(L.d3f_detection_scores(D(poisoned(x, m)), D(nbr), D(lengths), len(lengths), CAP, H, dim,
                                 P(out), P(ws), ws.numel(), _lib.stream(), D(dev_count(n, cuda))),
          "d3f_detection_scores")
     torch.cuda.synchronize()
-    ref = ok.detection_scores(x[:m].astype(np.float64), nbr[:m], lengths)
-    assert_close(out[:m].cpu().numpy(), ref, np.ones_like(ref), TOL, "detection_scores n=%d" % n)
+    ref, mag, alt = ok.detection_scores(x[:m].astype(np.float64), nbr[:m], lengths, magnitude=True)
+    assert_close(out[:real].cpu().numpy(), ref[:real], mag[:real], TOL, "detection_scores n=%d lengths %s" % (
+        n, "[%d]" % m if excess is None else "sum n%+d" % excess), alt=alt[:real])
     check_tail(out, m, "detection_scores")
+    if excess is not None and excess < 0:                          # the same clouds without the rows of no cloud
+        nb_real = np.where(nbr[:real] == m, real, nbr[:real])
+        ws = _lib.workspace(L.d3f_detection_scores_workspace_bytes(real, len(lengths)), cuda)
+        alone = torch.empty((real, 1), dtype=torch.float32, device=cuda)
+        call(L.d3f_detection_scores(D(x[:real]), D(nb_real), D(lengths), len(lengths), real, H, dim, P(alone), P(ws),
+                                    ws.numel(), _lib.stream(), None), "d3f_detection_scores")
+        torch.cuda.synchronize()
+        assert torch.equal(out[:real], alone), "rows past the last cloud changed a real row's score"

@@ -1,7 +1,8 @@
 """GPU parity for the rows SURVEY.md §8(f) marks "next": the detection score that is dumped next to the descriptors,
 neighbourhood calibration, and the deformable KITTI-shaped configuration at its full size (BASELINE.json configs[2]).
 
-Tolerances as in test_gpu_kpconv.py: 1e-4 max-norm relative on fp32 features, exact on integers.
+Tolerances as in test_gpu_kpconv.py: 1e-4 max-norm relative on fp32 features, exact on integers; the detection scores
+also element by element against float64 (tests/_oracle.py).
 """
 import numpy as np
 import pytest
@@ -9,6 +10,8 @@ import torch
 
 from oracle import native as on
 from oracle import kpconv_np as ok
+
+from _oracle import TOL, assert_close
 
 pytestmark = pytest.mark.gpu
 
@@ -25,24 +28,87 @@ def rel_err(a, b):
     return np.abs(a - b).max() / max(np.abs(b).max(), 1e-30)
 
 
-@pytest.mark.parametrize("lengths,D", [([1500, 1300], 32), ([700, 1, 900], 32), ([1200], 48)])
-def test_detection_scores_match_restatement(cuda, lengths, D):
-    """models/D3Feat.py:67-115 on random features: zero rows (count_nonzero), negative values, shadow neighbours."""
-    from d3feat_b200 import network_blocks as nb
-    rng = np.random.default_rng(7)
-    N = int(np.sum(lengths))
-    pts = np.concatenate([rng.uniform(0, 1, (n, 3)) for n in lengths]).astype(np.float32)
-    idx = on.port_batch_neighbors(pts, pts, lengths, lengths, 0.12, max_cols=30).astype(np.int32)
+SCORE_KINDS = ("plain", "steep", "negative_max", "cancelling", "max_near_minus_eps", "all_zero")
+
+
+def score_case(seed, lengths, D, H):
+    """Features [N, D], level-0 style neighbours [N, H] (shadow index N) and lengths for the detection scores. Cloud b
+    is of kind SCORE_KINDS[b % 6] (clouds of fewer than two rows stay plain):
+      plain               normal features, 10 % zero rows (a neighbour that does not vote)
+      steep               as plain, plus rows holding the cloud maximum in channel 0 whose other neighbours hold
+                          -(2..50) x that maximum there: d = f - mean from ~3 to past 20 (both softplus branches)
+      negative_max        every feature negative, so the cloud scale is negative
+      cancelling          as plain, plus rows whose channels cancel to an exactly zero sum in the kernel's
+                          warp-shuffle order and in numpy's pairwise order (D = 32 or 64; x[c + 8] = -x[c])
+      max_near_minus_eps  every feature negative with maximum ~ -1.05e-6: M + 1e-6 cancels to ~5e-8
+      all_zero            every feature zero (scale 1e6, score 0)
+    Neighbours: the row itself first, then random rows of its own cloud, 20 % shadow padding."""
+    rng = np.random.default_rng(seed)
+    lengths = np.asarray(lengths, np.int32)
+    N = int(lengths.sum())
+    start = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
     x = rng.normal(size=(N, D)).astype(np.float32)
-    x[rng.uniform(size=N) < 0.1] = 0.0                       # rows a ReLU-like block zeroed out
-    x[:, 3] = np.abs(x[:, 3])
-    ref = ok.detection_scores(x.astype(np.float64), idx, lengths)
-    out = nb.detection_scores(t(x, cuda), t(idx, cuda), t(np.asarray(lengths, np.int32), cuda)).cpu().numpy()
+    x[rng.uniform(size=N) < 0.1] = 0.0
+    nbr = np.full((N, H), N, np.int32)
+    for b, n in enumerate(lengths):
+        a, e = start[b], start[b + 1]
+        if n and H:
+            nbr[a:e] = rng.integers(a, e, (n, H))
+            nbr[a:e][rng.uniform(size=(n, H)) < 0.2] = N
+            nbr[a:e, 0] = np.arange(a, e)
+        kind = SCORE_KINDS[b % len(SCORE_KINDS)] if n >= 2 else "plain"
+        xb = x[a:e]
+        if kind == "steep" and H >= 2:
+            M = xb.max()
+            for r in rng.choice(n, min(n, 8), replace=False):
+                others = nbr[a + r, 1:]
+                others = others[(others < N) & (others != a + r)]
+                x[others, 0] = -rng.uniform(2, 50) * M
+            for r in rng.choice(n, min(n, 8), replace=False):
+                x[a + r, 0] = M
+        elif kind == "negative_max":
+            xb[:] = -np.abs(xb) - 0.25
+        elif kind == "cancelling" and D in (32, 64):
+            lo = np.arange(D)[(np.arange(D) & 8) == 0]
+            sel = rng.uniform(size=n) < 0.2
+            xb[np.ix_(sel, lo + 8)] = -xb[np.ix_(sel, lo)]
+        elif kind == "max_near_minus_eps":
+            xb[:] = -(np.abs(xb) + 1.05) * np.float32(1e-6)
+        elif kind == "all_zero":
+            xb[:] = 0.0
+    return x, nbr, lengths
+
+
+SCORE_CASES = {
+    # the three earlier (lengths, D) inputs, under the ids they have always had
+    "lengths0-32": ([1500, 1300], 32, 30), "lengths1-32": ([700, 1, 900], 32, 30), "lengths2-48": ([1200], 48, 30),
+    # many clouds, with empty and one-point clouds at the start, in the middle and at the end
+    "B17": ([0, 1, 300, 0, 0, 1, 250, 400, 1, 0, 350, 200, 1, 300, 280, 1, 0], 32, 24),
+    "B33": ([1, 0] + [37 * (i % 7) + (i % 3) for i in range(29)] + [0, 1], 32, 20),
+    "B300": ([(0, 1, 2, 17, 40, 5, 23)[i % 7] for i in range(300)], 32, 12),
+    # lane tails and several channels per lane
+    "D1": ([600, 0, 500, 400, 300, 350, 250], 1, 16),
+    "D31": ([600, 1, 500, 400, 300, 350, 250], 31, 16),
+    "D33": ([600, 500, 1, 400, 300, 350, 250], 33, 16),
+    "D64": ([600, 500, 450, 400, 300, 350, 250], 64, 16),
+    "H0": ([600, 500, 450, 400, 300, 350], 32, 0),
+    "H1": ([600, 500, 450, 400, 300, 350], 32, 1),
+}
+
+
+@pytest.mark.parametrize("case", sorted(SCORE_CASES))
+def test_detection_scores_match_restatement(cuda, case):
+    """models/D3Feat.py:67-115 against the float64 restatement, element by element (tests/_oracle.py): zero rows
+    (count_nonzero), negative values, shadow neighbours, and the clouds of score_case."""
+    from d3feat_b200 import network_blocks as nb
+    lengths, D, H = SCORE_CASES[case]
+    x, idx, lengths = score_case(sum(map(ord, case)), lengths, D, H)
+    N = x.shape[0]
+    ref, mag, alt = ok.detection_scores(x.astype(np.float64), idx, lengths, magnitude=True)
+    out = nb.detection_scores(t(x, cuda), t(idx, cuda), t(lengths, cuda)).cpu().numpy()
     assert out.shape == (N, 1)
     assert rel_err(out, ref) < RTOL
-    # the fp32 evaluation of the restatement agrees as well (same formula, numpy summation order)
-    ref32 = ok.detection_scores(x, idx, lengths)
-    assert rel_err(out, ref32) < RTOL
+    assert_close(out, ref, mag, TOL, "detection_scores %s" % case, alt=alt)
 
 
 def test_descriptors_and_scores_end_to_end(cuda):

@@ -1,13 +1,14 @@
-"""The element-wise check (tests/_oracle.py) is tight enough to matter: it rejects numpy emulations of the ways a KPConv
-or GEMM kernel typically goes wrong, at the shapes of the GPU tests, and accepts the float32 evaluation of the same
-restatement (what an honest fp32 kernel with another summation order computes). No GPU needed."""
+"""The element-wise check (tests/_oracle.py) is tight enough to matter: it rejects numpy emulations of the ways a KPConv,
+GEMM or detection-score kernel typically goes wrong, at the shapes of the GPU tests, and accepts the float32 evaluation
+of the same restatement (what an honest fp32 kernel with another summation order computes). No GPU needed."""
 import numpy as np
 import pytest
 
 from oracle import kpconv_np as ok
 
-from _oracle import TOL, assert_close, gemm_mag, epilogue, tf32, f64
+from _oracle import TOL, assert_close, gemm_mag, epilogue, ratio, tf32, f64
 from test_gpu_kpconv import make_case
+from test_gpu_widen import SCORE_CASES, score_case
 
 
 def rejects(out, ref, mag, alt=None):
@@ -166,3 +167,94 @@ def test_closest_mode_ties_are_marked():
     ref, mag, alt = ok.kpconv_ops(q, s, idx, f, Kp, W, 0.12, "linear", "closest", magnitude=True)
     assert not np.array_equal(ref[0], alt[0])
     assert np.array_equal(ref[1:], alt[1:]) or np.any(idx[1:] == sup)
+
+
+# ---- detection scores -------------------------------------------------------------------------------------------------
+
+SCORE_LENGTHS = [0, 1, 700, 600, 650, 500, 550, 450, 1, 0, 600, 520]    # every kind of score_case, twice over
+SCORE_BUGS = ("mean_over_h", "skip_last_column", "prev_cloud_max_first_row", "row_max", "softplus_cut_2")
+
+
+def _emulated_scores(x, nbr, lengths, bug=None):
+    """float32 emulation of the detection-score kernel (csrc/pool.cu): one scale 1/(M + 1e-6) per row applied to the
+    row and its neighbourhood, the count_nonzero vote on the raw row sum, one optional injected bug."""
+    f32 = np.float32
+    x = np.asarray(x, f32)
+    N, D = x.shape
+    start = np.concatenate([[0], np.cumsum(lengths)]).astype(np.int64)
+    cloud = np.searchsorted(start[1:], np.arange(N), side="right")
+    M = np.zeros(len(lengths), f32)
+    for b in range(len(lengths)):
+        if start[b + 1] > start[b]:
+            M[b] = x[start[b]:start[b + 1]].max()
+    if bug == "prev_cloud_max_first_row":
+        cloud = cloud[np.maximum(np.arange(N) - 1, 0)]            # the lookup shifted by one row
+    inv = f32(1) / (M[cloud] + f32(1e-6))
+    if bug == "row_max":
+        inv = f32(1) / (x.max(axis=1) + f32(1e-6))
+    inv = inv[:, None]
+    if bug == "skip_last_column":
+        nbr = nbr[:, :-1]
+    xs = np.concatenate([x, np.zeros((1, D), f32)], 0)
+    votes = np.concatenate([x.sum(axis=1) != 0, [False]])
+    cnt = np.maximum(votes[nbr].sum(axis=1), 1).astype(f32)[:, None]
+    if bug == "mean_over_h":
+        cnt = np.full_like(cnt, max(nbr.shape[1], 1))
+    f = x * inv
+    mean = (xs[nbr] * inv[:, :, None]).sum(axis=1) / cnt
+    d = f - mean
+    cut = f32(2) if bug == "softplus_cut_2" else f32(20)
+    sp = np.where(d > cut, d, np.log1p(np.exp(np.minimum(d, f32(20)))))
+    return (sp * (f / (f32(1e-6) + f.max(axis=1, keepdims=True)))).max(axis=1, keepdims=True)
+
+
+def test_detection_score_oracle_accepts_float32_and_rejects_bugs():
+    x, nbr, lengths = score_case(5, SCORE_LENGTHS, 32, 24)
+    ref, mag, alt = ok.detection_scores(f64(x), nbr, lengths, magnitude=True)
+    assert np.array_equal(ref, ok.detection_scores(f64(x), nbr, lengths))
+    rows = np.sort(np.random.default_rng(0).choice(x.shape[0], 500, replace=False))
+    r2, m2, a2 = ok.detection_scores(f64(x), nbr, lengths, magnitude=True, rows=rows, chunk=128)
+    assert np.array_equal(r2, ref[rows]) and np.array_equal(m2, mag[rows]) and np.array_equal(a2, alt[rows])
+    # the case reaches what it is built for: both softplus branches, and marked cancelling rows
+    assert (ref > 20).any() and ((ref > 2) & (ref < 20)).any()
+    assert not np.array_equal(ref, alt)
+    # honest float32 evaluations: the restatement in float32 and the kernel's own arithmetic, 10x inside the bar
+    worst = 0.0
+    for what, out in (("fp32 restatement", ok.detection_scores(x, nbr, lengths)),
+                      ("fp32 kernel emulation", _emulated_scores(x, nbr, lengths))):
+        worst = max(worst, assert_close(out, ref, mag, TOL / 10, "detection scores " + what, alt=alt))
+    print("detection scores: float32 headroom %.0fx (largest |err|/mag %.3e)" % (TOL / max(worst, 1e-300), worst))
+    weakest = None
+    for bug in SCORE_BUGS:
+        out = _emulated_scores(x, nbr, lengths, bug)
+        rejects(out, ref, mag, alt)
+        r = float(ratio(out, ref, mag, alt).max()) / TOL
+        print("detection scores, emulated bug %-26s largest |err|/mag = %.3g x TOL" % (bug, r))
+        weakest = r if weakest is None else min(weakest, r)
+    print("detection scores: weakest rejection %.3g x TOL" % weakest)
+
+
+def test_detection_score_oracle_cloud_bounds():
+    """Lengths summing to more than N cut the last cloud at N; rows past the last cloud belong to no cloud, so they do
+    not change any real row's score."""
+    x, nbr, lengths = score_case(6, [300, 0, 200, 250], 32, 12)
+    ref = ok.detection_scores(f64(x), nbr, lengths)
+    short = np.array([300, 0, 200, 200], np.int32)             # the last 50 rows belong to no cloud
+    big = x.copy()
+    big[700:] = 1e6
+    nb2 = nbr.copy()
+    nb2[(nb2 >= 700) & (nb2 < 750)] = 750                       # real rows do not reach them
+    got = ok.detection_scores(f64(big), nb2, short)
+    want = ok.detection_scores(f64(x[:700]), np.where(nb2[:700] == 750, 700, nb2[:700]), short)
+    assert np.array_equal(got[:700], want)
+    cut = ok.detection_scores(f64(x), nbr, np.array([300, 0, 200, 400], np.int32))
+    assert np.array_equal(cut, ref)
+
+
+@pytest.mark.parametrize("case", sorted(SCORE_CASES))
+def test_detection_score_emulation_accepted_on_every_gpu_case(case):
+    """The honest float32 kernel emulation passes the bar on every case test_detection_scores_match_restatement runs."""
+    lengths, D, H = SCORE_CASES[case]
+    x, nbr, lengths = score_case(sum(map(ord, case)), lengths, D, H)
+    ref, mag, alt = ok.detection_scores(f64(x), nbr, lengths, magnitude=True)
+    assert_close(_emulated_scores(x, nbr, lengths), ref, mag, TOL / 10, "fp32 kernel emulation " + case, alt=alt)
