@@ -47,6 +47,8 @@ SYMBOLS = [
     ("d3f_affine_leaky", _I, [_P, _I, _I, _P, _P, _P, _F, _P, _P, _P]),
     ("d3f_select_keypoints_workspace_bytes", _Z, [_I, _I]),
     ("d3f_select_keypoints", _I, [_P, _P, _I, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _Z, _P, _P]),
+    ("d3f_match_descriptors_workspace_bytes", _Z, [_I, _I]),
+    ("d3f_match_descriptors", _I, [_P, _P, _I, _I, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _Z, _P]),
 ]
 
 _lib = None

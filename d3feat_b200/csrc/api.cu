@@ -239,4 +239,13 @@ int d3f_select_keypoints(const float* scores, const int* lengths, int B, int N, 
                           out_descriptors, out_scores, workspace, workspace_bytes, (cudaStream_t)stream, n_dev);
 }
 
+size_t d3f_match_descriptors_workspace_bytes(int k, int P) { return match_descriptors_workspace_bytes(k, P); }
+
+int d3f_match_descriptors(const float* desc, const int* count, int B, int k, int D, const int* pairs, int P,
+                          int* nn_st, float* sim_st, int* nn_ts, float* sim_ts, int* matches, int* n_matches,
+                          void* workspace, size_t workspace_bytes, d3f_stream_t stream) {
+  return match_descriptors(desc, count, B, k, D, pairs, P, nn_st, sim_st, nn_ts, sim_ts, matches, n_matches, workspace,
+                           workspace_bytes, (cudaStream_t)stream);
+}
+
 }  // extern "C"

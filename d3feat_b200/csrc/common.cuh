@@ -66,6 +66,15 @@ __device__ __forceinline__ float ord2f(unsigned u) {
   return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
 }
 
+// order-preserving key of a canonicalised value: numpy's order for argsort / argmax. Every NaN (either sign) is one
+// positive quiet NaN above +inf; -0.0 equals +0.0, so the index decides. The key is never 0.
+__device__ __forceinline__ unsigned score_ord(float s) {
+  unsigned u = __float_as_uint(s);
+  if ((u & 0x7fffffffu) > 0x7f800000u) u = 0x7fc00000u;   // any NaN, either sign -> +qNaN (above +inf)
+  else if (u == 0x80000000u) u = 0u;                      // -0.0 -> +0.0 (numpy: equal, row order decides)
+  return f2ord(__uint_as_float(u));
+}
+
 // Row count of a launch: kernels are launched on a capacity-sized grid and read the actual number of rows from device
 // memory when the caller supplies it (the pyramid's level sizes are produced on the device; reading them back on the
 // host would put a synchronisation into every step). n_dev == nullptr: the capacity IS the row count.

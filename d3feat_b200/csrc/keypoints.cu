@@ -12,14 +12,6 @@
 
 namespace d3f {
 
-// order-preserving key of a canonicalised score
-__device__ __forceinline__ unsigned score_ord(float s) {
-  unsigned u = __float_as_uint(s);
-  if ((u & 0x7fffffffu) > 0x7f800000u) u = 0x7fc00000u;   // any NaN, either sign -> +qNaN (above +inf)
-  else if (u == 0x80000000u) u = 0u;                      // -0.0 -> +0.0 (numpy: equal, row order decides)
-  return f2ord(__uint_as_float(u));
-}
-
 // keys[i] = cloud(i) << 32 | ord(score[i]), vals[i] = i. Rows past the last cloud (lengths summing to less than n) get
 // cloud id B and sort behind every cloud.
 __global__ void __launch_bounds__(256)

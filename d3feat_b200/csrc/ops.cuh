@@ -101,4 +101,10 @@ int select_keypoints(const float* scores, const int* lengths, int B, int N, int 
                      float* out_descriptors, float* out_scores, void* workspace, size_t workspace_bytes,
                      cudaStream_t stream, const int* n_dev = nullptr);
 
+// ---- matching.cu ------------------------------------------------------------------------------------
+size_t match_descriptors_workspace_bytes(int k, int P);
+int match_descriptors(const float* desc, const int* count, int B, int k, int D, const int* pairs, int P, int* nn_st,
+                      float* sim_st, int* nn_ts, float* sim_ts, int* matches, int* n_matches, void* workspace,
+                      size_t workspace_bytes, cudaStream_t stream);
+
 }  // namespace d3f

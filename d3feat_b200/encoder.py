@@ -15,10 +15,13 @@ import torch
 from . import network_blocks as nb
 from . import pyramid
 from .keypoints import select_keypoints
+from .matching import host_pairs, match_keypoints
 from .variables import ParamStore, use_params
 
 # GraphPipeline(..., keypoints=k) result: descriptors [cap0,32], scores [cap0,1], keypoints (KeypointSet, k per cloud)
 Detections = namedtuple("Detections", "descriptors scores keypoints")
+# GraphPipeline(..., keypoints=k, match_pairs=pairs) result: the same plus matches (matching.Matches of every pair)
+MatchedDetections = namedtuple("MatchedDetections", "descriptors scores keypoints matches")
 
 
 class KPFCNN:
@@ -209,18 +212,27 @@ class GraphPipeline:
 
     keypoints=k (needs decoder=True): the encoder graph also runs the detection scores and the per-cloud top-k
     selection, and `res` is a Detections(descriptors [cap0,32], scores [cap0,1], keypoints) whose KeypointSet holds
-    the k highest-scoring level-0 points of every cloud -- slot buffers too, valid for the same DEPTH steps."""
+    the k highest-scoring level-0 points of every cloud -- slot buffers too, valid for the same DEPTH steps.
+
+    match_pairs=[(src, tgt), ...] (needs keypoints): the encoder graph then also matches the keypoint descriptors of
+    every pair (matching.match_keypoints), and `res` is a MatchedDetections(descriptors, scores, keypoints, matches).
+    The pairs are fixed for the pipeline: KITTI's tester is [(0, 1)], a 3DMatch scene batch every i < j."""
 
     DEPTH = 4
 
-    def __init__(self, enc, capacities, n_clouds, bbox, decoder=False, post=None, encoder_streams=2, keypoints=None):
+    def __init__(self, enc, capacities, n_clouds, bbox, decoder=False, post=None, encoder_streams=2, keypoints=None,
+                 match_pairs=None):
         if keypoints is not None and not decoder:
             raise ValueError("GraphPipeline: keypoints=%r needs decoder=True (the detection scores)" % (keypoints,))
         if keypoints is not None and int(keypoints) < 1:
             raise ValueError("GraphPipeline: keypoints=%r must be >= 1" % (keypoints,))
+        if match_pairs is not None and keypoints is None:
+            raise ValueError("GraphPipeline: match_pairs needs keypoints=k (the descriptors it matches)")
+        pairs = None if match_pairs is None else host_pairs(match_pairs, int(n_clouds), "GraphPipeline")
         self.keypoints = None if keypoints is None else int(keypoints)
         self.enc, self.decoder, self.post = enc, decoder, post
         dev = enc.device
+        self.match_pairs = None if pairs is None else torch.from_numpy(pairs).to(dev)
         self.caps = [int(c) for c in capacities]
         self.n_clouds = int(n_clouds)
         self.bbox = np.ascontiguousarray(bbox, np.float32)
@@ -265,6 +277,8 @@ class GraphPipeline:
             desc, scores = self.enc.describe(inputs, F, with_scores=True)
             kp = select_keypoints(scores, inputs["lengths"][0], self.keypoints, points=inputs["points"][0],
                                   descriptors=desc, rows=inputs["rows"][0])
+            if self.match_pairs is not None:
+                return F, MatchedDetections(desc, scores, kp, match_keypoints(kp, self.match_pairs))
             return F, Detections(desc, scores, kp)
         res = self.enc.describe(inputs, F) if self.decoder else F[-1]
         return F, res

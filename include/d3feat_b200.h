@@ -26,6 +26,8 @@
  *   d3f_closest_pool          models/network_blocks.py:69-83
  *   d3f_l2_normalize          models/D3Feat.py:65
  *   d3f_select_keypoints      utils/tester.py:209-213, 281-290 (host argsort of the detection scores)
+ *   d3f_match_descriptors     geometric_registration/evaluate.py:11-27 (build_correspondence: mutual nearest
+ *                             neighbours of two fragments' keypoint descriptors)
  */
 #ifndef D3FEAT_B200_H_
 #define D3FEAT_B200_H_
@@ -273,6 +275,27 @@ int d3f_select_keypoints(const float* scores, const int* lengths, int B, int N, 
                          const float* descriptors, int D, int* out_order, int* out_index, int* out_count,
                          float* out_points, float* out_descriptors, float* out_scores, void* workspace,
                          size_t workspace_bytes, d3f_stream_t stream, const int* n_dev);
+
+/* Descriptor matching between the keypoint sets of P cloud pairs (geometric_registration/evaluate.py:11-27).
+ *   desc[B,k,D], count[B] (device) in the d3f_select_keypoints layout: slot j of cloud b is real iff
+ *   j < clamp(count[b], 0, k). pairs[P,2] (device) = (src cloud, tgt cloud).
+ *   For pair p with a = desc[src, :n_s], b = desc[tgt, :n_t]:
+ *     s_ij = 0.0f, then for c = 0 .. D-1 in ascending order s_ij = fadd_rn(s_ij, fmul_rn(a_ic, b_jc)) -- fp32, no FMA.
+ *     nn_st[p,i] = argmax_j s_ij, sim_st[p,i] = s[i, nn_st[p,i]]; nn_ts[p,j] = argmax_i s_ij, sim_ts likewise.
+ *     argmax has numpy's semantics: NaN above everything, -0.0 equal to +0.0, ties to the smallest slot. A NaN
+ *     similarity is reported as the positive quiet NaN 0x7fc00000.
+ *     matches[p,m,:] = (i, nn_st[p,i]) for every real i with nn_ts[p, nn_st[p,i]] == i, in ascending i;
+ *     n_matches[p] = their number. Unused match rows hold -1.
+ *   Slots i >= n_s get nn = -1 and sim = 0, and so does every slot when the other cloud is empty. Slots at or past
+ *   the count are never read; neither is a cloud outside [0, B), and a pair naming one matches nothing.
+ *   On unit descriptors argmax s is the reference's argmin sqrt(2 - 2s), except where the rounding of 2 - 2s merges
+ *   distinct similarities.
+ *   Returns D3F_ERR_INVALID for B outside [1, 1024], k < 1, D < 1, P < 1, P*k beyond int32 or a null pointer (every
+ *   output is required), D3F_ERR_WORKSPACE for a short workspace. Graph-capturable. */
+size_t d3f_match_descriptors_workspace_bytes(int k, int P);
+int d3f_match_descriptors(const float* desc, const int* count, int B, int k, int D, const int* pairs, int P,
+                          int* nn_st, float* sim_st, int* nn_ts, float* sim_ts, int* matches, int* n_matches,
+                          void* workspace, size_t workspace_bytes, d3f_stream_t stream);
 
 #ifdef __cplusplus
 }
