@@ -15,6 +15,7 @@ LIB_PATH = os.environ.get("D3F_LIB") or os.path.join(_HERE, "libd3feat_b200.so")
 
 # every symbol include/d3feat_b200.h declares: (name, restype, argtypes)
 _P, _I, _F, _Z, _LL = C.c_void_p, C.c_int, C.c_float, C.c_size_t, C.c_longlong
+_D, _U64 = C.c_double, C.c_uint64
 SYMBOLS = [
     ("d3f_version", _I, []),
     ("d3f_last_error", C.c_char_p, []),
@@ -49,6 +50,9 @@ SYMBOLS = [
     ("d3f_select_keypoints", _I, [_P, _P, _I, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _Z, _P, _P]),
     ("d3f_match_descriptors_workspace_bytes", _Z, [_I, _I]),
     ("d3f_match_descriptors", _I, [_P, _P, _I, _I, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _Z, _P]),
+    ("d3f_register_pairs_workspace_bytes", _Z, [_I, _I, _I, _I]),
+    ("d3f_register_pairs", _I, [_P, _P, _I, _I, _P, _P, _I, _P, _I, _I, _I, _I, _D, _D, _U64, _P, _P, _P, _P, _P, _Z,
+                                _P]),
 ]
 
 _lib = None

@@ -248,4 +248,17 @@ int d3f_match_descriptors(const float* desc, const int* count, int B, int k, int
                            workspace_bytes, (cudaStream_t)stream);
 }
 
+size_t d3f_register_pairs_workspace_bytes(int L, int P, int max_iterations, int max_validation) {
+  return register_pairs_workspace_bytes(L, P, max_iterations, max_validation);
+}
+
+int d3f_register_pairs(const float* points, const int* count, int B, int k, const int* corr, const int* n_corr, int L,
+                       const int* pairs, int P, int ransac_n, int max_iterations, int max_validation, double distance,
+                       double edge_ratio, unsigned long long seed, double* pose, int* n_inliers, int* hypothesis,
+                       int* n_validated, void* workspace, size_t workspace_bytes, d3f_stream_t stream) {
+  return register_pairs(points, count, B, k, corr, n_corr, L, pairs, P, ransac_n, max_iterations, max_validation,
+                        distance, edge_ratio, seed, pose, n_inliers, hypothesis, n_validated, workspace,
+                        workspace_bytes, (cudaStream_t)stream);
+}
+
 }  // extern "C"

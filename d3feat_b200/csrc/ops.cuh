@@ -107,4 +107,11 @@ int match_descriptors(const float* desc, const int* count, int B, int k, int D, 
                       float* sim_st, int* nn_ts, float* sim_ts, int* matches, int* n_matches, void* workspace,
                       size_t workspace_bytes, cudaStream_t stream);
 
+// ---- registration.cu --------------------------------------------------------------------------------
+size_t register_pairs_workspace_bytes(int L, int P, int max_iterations, int max_validation);
+int register_pairs(const float* points, const int* count, int B, int k, const int* corr, const int* n_corr, int L,
+                   const int* pairs, int P, int ransac_n, int max_iterations, int max_validation, double distance,
+                   double edge_ratio, unsigned long long seed, double* pose, int* n_inliers, int* hypothesis,
+                   int* n_validated, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+
 }  // namespace d3f

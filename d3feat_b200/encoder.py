@@ -16,12 +16,15 @@ from . import network_blocks as nb
 from . import pyramid
 from .keypoints import select_keypoints
 from .matching import host_pairs, match_keypoints
+from .registration import OPTIONS as REGISTER_OPTIONS, check_options, register_pairs
 from .variables import ParamStore, use_params
 
 # GraphPipeline(..., keypoints=k) result: descriptors [cap0,32], scores [cap0,1], keypoints (KeypointSet, k per cloud)
 Detections = namedtuple("Detections", "descriptors scores keypoints")
 # GraphPipeline(..., keypoints=k, match_pairs=pairs) result: the same plus matches (matching.Matches of every pair)
 MatchedDetections = namedtuple("MatchedDetections", "descriptors scores keypoints matches")
+# GraphPipeline(..., match_pairs=pairs, register={...}) result: the same plus registration (registration.Registration)
+RegisteredDetections = namedtuple("RegisteredDetections", "descriptors scores keypoints matches registration")
 
 
 class KPFCNN:
@@ -216,19 +219,31 @@ class GraphPipeline:
 
     match_pairs=[(src, tgt), ...] (needs keypoints): the encoder graph then also matches the keypoint descriptors of
     every pair (matching.match_keypoints), and `res` is a MatchedDetections(descriptors, scores, keypoints, matches).
-    The pairs are fixed for the pipeline: KITTI's tester is [(0, 1)], a 3DMatch scene batch every i < j."""
+    The pairs are fixed for the pipeline: KITTI's tester is [(0, 1)], a 3DMatch scene batch every i < j.
+
+    register={...} (needs match_pairs): the keyword arguments of registration.register_pairs ({} for the 3DMatch
+    evaluation's defaults). The encoder graph then also estimates every pair's pose by RANSAC over its matches, and
+    `res` is a RegisteredDetections(descriptors, scores, keypoints, matches, registration)."""
 
     DEPTH = 4
 
     def __init__(self, enc, capacities, n_clouds, bbox, decoder=False, post=None, encoder_streams=2, keypoints=None,
-                 match_pairs=None):
+                 match_pairs=None, register=None):
         if keypoints is not None and not decoder:
             raise ValueError("GraphPipeline: keypoints=%r needs decoder=True (the detection scores)" % (keypoints,))
         if keypoints is not None and int(keypoints) < 1:
             raise ValueError("GraphPipeline: keypoints=%r must be >= 1" % (keypoints,))
         if match_pairs is not None and keypoints is None:
             raise ValueError("GraphPipeline: match_pairs needs keypoints=k (the descriptors it matches)")
+        if register is not None:
+            if match_pairs is None:
+                raise ValueError("GraphPipeline: register needs match_pairs (the matches it registers)")
+            if not isinstance(register, dict) or set(register) - set(REGISTER_OPTIONS):
+                raise ValueError("GraphPipeline: register must be a dict of register_pairs options %s, got %r" % (
+                    REGISTER_OPTIONS, register))
+            check_options(**register, who="GraphPipeline")
         pairs = None if match_pairs is None else host_pairs(match_pairs, int(n_clouds), "GraphPipeline")
+        self.register = None if register is None else dict(register)
         self.keypoints = None if keypoints is None else int(keypoints)
         self.enc, self.decoder, self.post = enc, decoder, post
         dev = enc.device
@@ -278,7 +293,11 @@ class GraphPipeline:
             kp = select_keypoints(scores, inputs["lengths"][0], self.keypoints, points=inputs["points"][0],
                                   descriptors=desc, rows=inputs["rows"][0])
             if self.match_pairs is not None:
-                return F, MatchedDetections(desc, scores, kp, match_keypoints(kp, self.match_pairs))
+                m = match_keypoints(kp, self.match_pairs)
+                if self.register is not None:
+                    reg = register_pairs(kp, m, self.match_pairs, **self.register)
+                    return F, RegisteredDetections(desc, scores, kp, m, reg)
+                return F, MatchedDetections(desc, scores, kp, m)
             return F, Detections(desc, scores, kp)
         res = self.enc.describe(inputs, F) if self.decoder else F[-1]
         return F, res

@@ -28,6 +28,9 @@
  *   d3f_select_keypoints      utils/tester.py:209-213, 281-290 (host argsort of the detection scores)
  *   d3f_match_descriptors     geometric_registration/evaluate.py:11-27 (build_correspondence: mutual nearest
  *                             neighbours of two fragments' keypoint descriptors)
+ *   d3f_register_pairs        geometric_registration/evaluate.py:84-99, utils/tester.py:305-316,
+ *                             demo_registration.py:184-192 (Open3D's RANSAC over the keypoint correspondences,
+ *                             with the edge-length and distance checkers)
  */
 #ifndef D3FEAT_B200_H_
 #define D3FEAT_B200_H_
@@ -296,6 +299,37 @@ size_t d3f_match_descriptors_workspace_bytes(int k, int P);
 int d3f_match_descriptors(const float* desc, const int* count, int B, int k, int D, const int* pairs, int P,
                           int* nn_st, float* sim_st, int* nn_ts, float* sim_ts, int* matches, int* n_matches,
                           void* workspace, size_t workspace_bytes, d3f_stream_t stream);
+
+/* Rigid registration of P cloud pairs by deterministic RANSAC over keypoint correspondences
+ * (geometric_registration/evaluate.py:84-99, utils/tester.py:305-316, demo_registration.py:184-192, which call
+ * Open3D's registration_ransac_based_on_* with CorrespondenceCheckerBasedOnEdgeLength / OnDistance).
+ *   points[B,k,3] fp32, count[B] (device) in the d3f_select_keypoints layout: slot j of cloud b is real iff
+ *   j < clamp(count[b], 0, k). pairs[P,2] (device) = (src cloud, tgt cloud). corr[P,L,2] (device) = (source slot,
+ *   target slot) rows, of which the first n_c = clamp(n_corr[p], 0, L) are real.
+ *   Contract (exact; oracle/register_np.py restates it in numpy): every step is one correctly rounded fp64 operation
+ *   in a fixed order (no fused multiply-add), sums sequential in ascending index, points widened from fp32 exactly.
+ *     hypothesis h in [0, max_iterations) samples idx_m, m < ransac_n: c = ((p << 32) | h) * 8 + m,
+ *       z = splitmix64(seed + c * 0x9E3779B97F4A7C15), idx_m = ((z >> 32) * n_c) >> 32 (uint64, wrapping);
+ *       a repeated index rejects it; the edge checker rejects it if |s_a - s_b| < edge_ratio * |t_a - t_b| or the
+ *       reverse for any a < b; the pose is Horn's quaternion method (centroids, centred cross-covariance, cyclic
+ *       Jacobi on the 4x4 matrix, 6 sweeps, exact-zero pivots skipped); every sample row must then have
+ *       |R s + t - t'|^2 <= distance^2. Only the first max_validation validated hypotheses in ascending h are scored.
+ *     A row is an inlier if |R s + t - t'|^2 < distance^2. The best hypothesis has the most inliers, then the smaller
+ *     sequential sum of inlier d^2, then the smaller h; the pose is refit over its inliers in ascending row order
+ *     (kept as it is if it has none).
+ *   Outputs: pose[P,4,4] fp64 (t' ~ R s + t, row-major, last row 0 0 0 1), n_inliers[P], hypothesis[P] (the best h)
+ *   and n_validated[P] (the number scored). A pair naming a cloud outside [0, B), or with a real row naming a slot at
+ *   or past its cloud's count, registers nothing and reads neither; so does a pair with n_c < ransac_n or without a
+ *   validated hypothesis: identity, 0, -1 and its validated count.
+ *   Limits: B in [1, 1024]; k, L, P >= 1; ransac_n in [3, 8]; max_iterations in [1, 2^24]; max_validation in
+ *   [1, max_iterations]; distance finite and > 0; edge_ratio in (0, 1]; B*k*3, P*L*2 and P*max_iterations within
+ *   int32. Otherwise, or for a null pointer, D3F_ERR_INVALID before any CUDA call; D3F_ERR_WORKSPACE for a short
+ *   workspace. Graph-capturable: counts, n_corr and pair ids are read on the device. */
+size_t d3f_register_pairs_workspace_bytes(int L, int P, int max_iterations, int max_validation);
+int d3f_register_pairs(const float* points, const int* count, int B, int k, const int* corr, const int* n_corr, int L,
+                       const int* pairs, int P, int ransac_n, int max_iterations, int max_validation, double distance,
+                       double edge_ratio, unsigned long long seed, double* pose, int* n_inliers, int* hypothesis,
+                       int* n_validated, void* workspace, size_t workspace_bytes, d3f_stream_t stream);
 
 #ifdef __cplusplus
 }
