@@ -84,6 +84,15 @@ __device__ __forceinline__ int dyn_rows(int n_cap, const int* __restrict__ n_dev
   return n < n_cap ? (n < 0 ? 0 : n) : n_cap;
 }
 
+// Rows of a stacked batch that belong to a cloud: the row count cut at start[B]. Rows at or past start[B] (lengths
+// summing to less than the row count) belong to no cloud; lengths summing to more cut the last cloud at the row count.
+__device__ __forceinline__ int cloud_rows(int n_cap, const int* __restrict__ n_dev, const int* __restrict__ start,
+                                          int B) {
+  const int n = dyn_rows(n_cap, n_dev);
+  const int e = start[B];
+  return e < n ? (e < 0 ? 0 : e) : n;
+}
+
 // batch element of a stacked row index: largest b with start[b] <= i (start = exclusive scan of lengths)
 __device__ __forceinline__ int batch_of(const int* __restrict__ start, int B, int i) {
   int lo = 0, hi = B - 1;

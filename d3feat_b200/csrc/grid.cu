@@ -50,11 +50,14 @@ int launch_batch_start(const int* len, int B, int* start, cudaStream_t stream) {
 }
 
 // bbox_ord[b*6 + {0,1,2}] = min (ordered uint), [3,4,5] = max. Must be pre-set to 0xFF.. / 0.
+// With `start`, only the rows that belong to a cloud are visited, and their number goes to *n_rows (the row count of
+// every later kernel of the subsampling).
 __global__ void __launch_bounds__(256) bbox_batch_kernel(const float* __restrict__ pts, int Ncap,
                                                          const int* __restrict__ n_dev,
                                                          const int* __restrict__ start, int B,
-                                                         unsigned* __restrict__ bbox_ord) {
-  const int N = dyn_rows(Ncap, n_dev);
+                                                         unsigned* __restrict__ bbox_ord, int* __restrict__ n_rows) {
+  const int N = start != nullptr ? cloud_rows(Ncap, n_dev, start, B) : dyn_rows(Ncap, n_dev);
+  if (n_rows != nullptr && blockIdx.x == 0 && threadIdx.x == 0) *n_rows = N;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < ceil_div(N, 32) * 32; i += gridDim.x * blockDim.x) {
     bool valid = i < N;
     int b = valid ? batch_of(start, B, i) : -1;
@@ -102,7 +105,7 @@ int bbox_device(const float* pts, int N, float* out_bbox, cudaStream_t stream) {
   D3F_CUDA(cudaMemsetAsync(ord + 3, 0, 3 * sizeof(unsigned), stream));
   if (N > 0) {
     int blocks = min(ceil_div(N, 256), kNumSMs * 4);
-    bbox_batch_kernel<<<blocks, 256, 0, stream>>>(pts, N, nullptr, nullptr, 1, ord);
+    bbox_batch_kernel<<<blocks, 256, 0, stream>>>(pts, N, nullptr, nullptr, 1, ord, nullptr);
     D3F_LAUNCH_CHECK("bbox_batch_kernel");
   }
   bbox_decode_kernel<<<1, 32, 0, stream>>>(ord, out_bbox, 6);
@@ -220,7 +223,7 @@ cell_feature_kernel(const float* __restrict__ feats, int fdim, const uint32_t* _
   out_feats[(size_t)m * fdim + c] = __fdiv_rn(s, (float)count);
 }
 
-// a sort-key overflow (points outside the host bbox) is reported to the caller as out_M = -1, more cells than the
+// a sort-key overflow (a cloud wider than the host bbox allows) is reported to the caller as out_M = -1, more cells than the
 // output capacity as out_M = -2; `status` (optional) accumulates the same conditions as bits 1 / 2 for callers that
 // never read out_M on the host (the graph-replayed pyramid)
 __global__ void subsample_status_kernel(const int* __restrict__ err, int* __restrict__ out_M, int out_cap,
@@ -257,6 +260,7 @@ struct SubsampleWs {
   int* cell_first;
   int* cell_count;
   int* err;
+  int* n_rows;   // rows that belong to a cloud: min(row count, start[B]), written by bbox_batch_kernel
 };
 
 static size_t carve_subsample(Carver& cv, int N, int B, SubsampleWs& w) {
@@ -274,6 +278,7 @@ static size_t carve_subsample(Carver& cv, int N, int B, SubsampleWs& w) {
   w.cell_first = cv.take<int>(n);
   w.cell_count = cv.take<int>(n);
   w.err = cv.take<int>(1);
+  w.n_rows = cv.take<int>(1);
   return cv.off;
 }
 
@@ -318,20 +323,21 @@ int grid_subsample(const float* pts, const int* batch_len, int B, int N, float d
     // min slots to 0xFFFFFFFF via a strided 2D memset: rows of 6 uints, first 3 set
     D3F_CUDA(cudaMemset2DAsync(w.bbox_ord, 6 * sizeof(unsigned), 0xff, 3 * sizeof(unsigned), B, stream));
   }
+  // rows at or past start[B] belong to no cloud: from here on every kernel's row count is w.n_rows
   int blocks = min(ceil_div(N, 256), kNumSMs * 8);
-  bbox_batch_kernel<<<blocks, 256, 0, stream>>>(pts, N, n_dev, w.start, B, w.bbox_ord);
+  bbox_batch_kernel<<<blocks, 256, 0, stream>>>(pts, N, n_dev, w.start, B, w.bbox_ord, w.n_rows);
   D3F_LAUNCH_CHECK("bbox_batch_kernel");
-  cell_key_kernel<<<ceil_div(N, 256), 256, 0, stream>>>(pts, N, n_dev, w.start, B, w.bbox_ord, dl, cell_bits,
+  cell_key_kernel<<<ceil_div(N, 256), 256, 0, stream>>>(pts, N, w.n_rows, w.start, B, w.bbox_ord, dl, cell_bits,
                                                         w.sort.keys[0], w.sort.vals[0], w.err);
   D3F_LAUNCH_CHECK("cell_key_kernel");
-  int cur = radix_sort_pairs(w.sort, N, cell_bits + 1 + bbits, stream, n_dev);
+  int cur = radix_sort_pairs(w.sort, N, cell_bits + 1 + bbits, stream, w.n_rows);
   if (cur < 0) return cur;
-  segment_head_kernel<<<ceil_div(N, 256), 256, 0, stream>>>(w.sort.keys[cur], N, n_dev, w.flags);
+  segment_head_kernel<<<ceil_div(N, 256), 256, 0, stream>>>(w.sort.keys[cur], N, w.n_rows, w.flags);
   D3F_LAUNCH_CHECK("segment_head_kernel");
-  int rc = exclusive_scan_i32(w.flags, w.cell_of, N, out_M, w.scan_scratch, stream, n_dev);
+  int rc = exclusive_scan_i32(w.flags, w.cell_of, N, out_M, w.scan_scratch, stream, w.n_rows);
   if (rc) return rc;
   cell_reduce_kernel<<<ceil_div(N, 128), 128, 0, stream>>>(pts, w.sort.keys[cur], w.sort.vals[cur], w.flags,
-                                                           w.cell_of, N, n_dev, out_capacity, cell_bits, classes,
+                                                           w.cell_of, N, w.n_rows, out_capacity, cell_bits, classes,
                                                            ldim, out_pts, out_classes, out_batch_len, w.cell_first,
                                                            w.cell_count);
   D3F_LAUNCH_CHECK("cell_reduce_kernel");

@@ -47,12 +47,13 @@ __device__ __forceinline__ int cell_coord(float v, float mn, float inv, int n) {
 
 // Grid build = counting sort by cell: (1) count points per cell, (2) exclusive scan -> cell_start (cell c owns
 // [cell_start[c], cell_start[c+1])), (3) scatter. The order of the points INSIDE a cell is whatever the atomics give;
-// no result depends on it (rows are emitted in (d2, index) order).
+// no result depends on it (rows are emitted in (d2, index) order). Supports at or past start[B] belong to no cloud and
+// enter no cell.
 __global__ void __launch_bounds__(256)
 cell_count_kernel(const float* __restrict__ s, int Ns_cap, const int* __restrict__ ns_dev,
                   const int* __restrict__ start, int B, NbGrid g, uint32_t* __restrict__ cell_id,
                   int* __restrict__ cell_cnt) {
-  const int Ns = dyn_rows(Ns_cap, ns_dev);
+  const int Ns = cloud_rows(Ns_cap, ns_dev, start, B);
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= Ns) return;
   int b = batch_of(start, B, i);
@@ -64,16 +65,16 @@ cell_count_kernel(const float* __restrict__ s, int Ns_cap, const int* __restrict
   atomicAdd(&cell_cnt[c], 1);
 }
 
-// sorted_pts[pos] = (x, y, z, bits(index)); cell_cnt is counted back down to zero
+// sorted_pts[pos] = (x, y, z, bits(index)); cell_cnt is counted back down to zero. A support of no cloud keeps its own
+// position, past every cell's run, so that the cell order stays a permutation of the rows.
 __global__ void __launch_bounds__(256)
 cell_scatter_kernel(const float* __restrict__ s, int Ns_cap, const int* __restrict__ ns_dev,
-                    const uint32_t* __restrict__ cell_id, const int* __restrict__ cell_start,
-                    int* __restrict__ cell_cnt, float4* __restrict__ sorted_pts) {
+                    const int* __restrict__ start, int B, const uint32_t* __restrict__ cell_id,
+                    const int* __restrict__ cell_start, int* __restrict__ cell_cnt, float4* __restrict__ sorted_pts) {
   const int Ns = dyn_rows(Ns_cap, ns_dev);
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= Ns) return;
-  uint32_t c = cell_id[i];
-  int pos = cell_start[c] + atomicSub(&cell_cnt[c], 1) - 1;
+  const int pos = i < start[B] ? cell_start[cell_id[i]] + atomicSub(&cell_cnt[cell_id[i]], 1) - 1 : i;
   sorted_pts[pos] = make_float4(s[3 * (size_t)i], s[3 * (size_t)i + 1], s[3 * (size_t)i + 2], __uint_as_float((uint32_t)i));
 }
 
@@ -142,8 +143,8 @@ int radius_neighbors_build(const float* supports, const int* s_batch_len, int B,
   D3F_LAUNCH_CHECK("cell_count_kernel");
   if (exclusive_scan_i32(w.cell_cnt, w.cell_start, (int)total, w.cell_start + total, w.scan_scratch, stream))
     return D3F_ERR_CUDA;
-  cell_scatter_kernel<<<ceil_div(Ns, 256), 256, 0, stream>>>(supports, Ns, ns_dev, w.cell_id, w.cell_start, w.cell_cnt,
-                                                             w.sorted_pts);
+  cell_scatter_kernel<<<ceil_div(Ns, 256), 256, 0, stream>>>(supports, Ns, ns_dev, w.s_start, B, w.cell_id, w.cell_start,
+                                                             w.cell_cnt, w.sorted_pts);
   D3F_LAUNCH_CHECK("cell_scatter_kernel");
   return D3F_OK;
 }
@@ -256,7 +257,8 @@ radius_query_kernel(const float* __restrict__ q, int Nq_cap, const int* __restri
     if (lane >= o) inc += t;
   }
   if (lane < 9) run_tab[warp][lane] = make_int2(inc, rs - (inc - rl));
-  const int T = __shfl_sync(0xffffffffu, inc, 8);
+  int T = __shfl_sync(0xffffffffu, inc, 8);
+  if (qi >= __ldg(q_start + B)) T = 0;   // a query of no cloud: no neighbours, a row of padding
   if (lane == 9) run_tab[warp][9] = make_int2(0x7fffffff, 0);   // sentinel: the walk below never runs off the table
   __syncwarp();
 
@@ -507,7 +509,7 @@ radius_query2_kernel(const float* __restrict__ q, int Nq_cap, const int* __restr
   }
   if (hl < 9) run_tab[slot][hl] = make_int2(inc, rs - (inc - rl));
   int T = __shfl_sync(0xffffffffu, inc, 8, 16);
-  if (!qvalid) T = 0;
+  if (!qvalid || qi >= __ldg(q_start + B)) T = 0;   // a query of no cloud: no neighbours, a row of padding
   if (hl == 9) run_tab[slot][9] = make_int2(0x7fffffff, 0);
   __syncwarp();
   const int Tmax = max(T, __shfl_xor_sync(0xffffffffu, T, 16));
@@ -678,6 +680,7 @@ int radius_neighbors_count(const float* queries, const int* q_batch_len, int Nq,
 int radius_neighbors_fill(const float* queries, const int* q_batch_len, int Nq, int B, int Ns, float radius,
                           const float* host_bbox, const void* workspace, int cols, int pad_value, int* out_idx,
                           cudaStream_t stream, const int* nq_dev, const int* pad_dev, const int* q_start_pre) {
+  D3F_REQUIRE(B >= 1 && B <= kMaxBatch, D3F_ERR_INVALID, "radius_neighbors: B=%d must be in [1,%d]", B, kMaxBatch);
   D3F_REQUIRE(cols >= 0 && (out_idx != nullptr || cols == 0 || Nq == 0), D3F_ERR_INVALID,
               "radius_neighbors_fill: cols=%d / null output", cols);
   if (cols == 0) return D3F_OK;

@@ -62,7 +62,7 @@ __global__ void set_count_kernel(int* __restrict__ dst, int value, const int* __
 //    synchronisation per level) so that the next level's launches and the caller's tensor views have exact sizes --
 //    what the TF ops do, and what the stand-alone op mirrors / parity tests use;
 //  * static (out_level_sizes == nullptr): nothing is read back. Every launch is sized by capacity[l], every kernel
-//    takes its row count from d_counts[l] in device memory, errors (more cells than capacity[l+1], points outside the
+//    takes its row count from d_counts[l] in device memory, errors (more cells than capacity[l+1], a cloud wider than the
 //    bbox) are OR-ed into *d_status. The launch sequence then depends on nothing but (B, capacity, spec, bbox): it
 //    can be captured once as a CUDA graph and replayed for every batch of the bucket.
 // d_counts[0] is N0, or *n0_dev when the caller keeps the level-0 count on the device (graph replay: N0 = capacity[0]).
@@ -160,7 +160,7 @@ int pyramid_build(const float* points, const int* lengths, int B, int N0, const 
       if (exact) {
         D3F_CUDA(cudaMemcpyAsync(&M, d_M, sizeof(int), cudaMemcpyDeviceToHost, stream));
         D3F_CUDA(cudaStreamSynchronize(stream));
-        D3F_REQUIRE(M != -1, D3F_ERR_CAPACITY, "pyramid_build: points fall outside the supplied bbox at level %d", l);
+        D3F_REQUIRE(M != -1, D3F_ERR_CAPACITY, "pyramid_build: a cloud at level %d is wider than the supplied bbox allows", l);
         D3F_REQUIRE(M >= 0, D3F_ERR_CAPACITY, "pyramid_build: level %d exceeds its capacity %d", l + 1, capacity[l + 1]);
       }
       lvl_pts[l + 1] = out_points[l + 1];

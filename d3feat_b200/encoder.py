@@ -396,4 +396,4 @@ class GraphPipeline:
             st = int(buf.status.item())
             if st:
                 raise RuntimeError("GraphPipeline: slot %d status %d (%s)" % (
-                    k, st, "points outside the scene bounds" if st & 1 else "a level exceeded its capacity"))
+                    k, st, "a cloud wider than the scene bounds" if st & 1 else "a level exceeded its capacity"))

@@ -150,7 +150,7 @@ def _subsample(points, batches, dl, features=None, classes=None, bbox=None, sync
                                     _lib.ptr(out_m), _lib.ptr(ws), ws.numel(), _lib.stream()), "d3f_grid_subsample")
     M = int(out_m.item())
     if M < 0:
-        raise _lib.D3FError("grid_subsample: points fall outside the supplied bbox (sort-key overflow)")
+        raise _lib.D3FError("grid_subsample: a cloud is wider than the supplied bbox allows (sort-key overflow)")
     res = [out_p[:M], out_b]
     if fdim:
         res.append(out_f[:M])

@@ -72,8 +72,13 @@ int d3f_bbox(const float* pts, int N, float* out_bbox, d3f_stream_t stream);
  * Grid subsampling (voxel barycenters), stacked clouds.
  *   pts[N,3], batch_len[B] (device int32), dl: cell size.
  *   feats[N,fdim] / classes[N,ldim] optional (NULL, 0): the cpp_wrappers signature.
+ *   Row i belongs to cloud b when start[b] <= i < start[b+1] (start = exclusive scan of batch_len). Rows at or
+ *     past start[B] (lengths summing to less than N) belong to no cloud and are never read; lengths summing to more
+ *     than N cut the last cloud at N.
  *   host_bbox: host float[6] bounding ALL points (from d3f_bbox or known a priori). It only bounds
- *     the sort-key width; the per-cloud origin is recomputed exactly on the device.
+ *     the sort-key width; the per-cloud origin is recomputed exactly on the device. A cloud merely displaced
+ *     outside host_bbox is still subsampled exactly; a cloud whose own extent needs more cells than host_bbox
+ *     allows overflows the sort key and is reported as out_M = -1.
  *   Outputs (capacity N rows each): out_pts[<=N,3], out_feats, out_classes, out_batch_len[B],
  *     out_M[1] (device int32: total number of cells). Cells are emitted per cloud in ascending
  *     reference cell key iX + NX*iY + NX*NY*iZ (grid_subsampling.cpp:53-56); barycenters are
@@ -94,6 +99,10 @@ int d3f_grid_subsample(const float* pts, const int* batch_len, int B, int N, flo
  *   supports of the same cloud with d2 < radius*radius, d2 = ((dx*dx)+dy*dy)+dz*dz in fp32 without
  *   FMA contraction, rows sorted by ascending (d2, index), global support indices, rows padded with
  *   pad_value (Ns for the batch op, -1 for the non-batch op).
+ *   Clouds as in d3f_grid_subsample: supports at or past the end of the last support cloud are in no cloud and
+ *   never returned; a query at or past the end of the last query cloud gets count 0 and a row of padding; lengths
+ *   summing past the row count cut the last cloud there. host_bbox sizes the grid; points outside it are clamped
+ *   into its edge cells, which only adds candidates, so results stay exact.
  *
  *   Two-phase use for the exact reference shape [Nq, max count]:
  *     d3f_radius_neighbors_build  -> grid over the supports in `workspace`
@@ -127,14 +136,17 @@ int d3f_radius_neighbors_fill(const float* queries, const int* q_batch_len, int 
  * if sub_dl[l] > 0: points_{l+1} = grid_subsample(points_l, sub_dl[l]); pools[l] = search(points_{l+1}, points_l,
  * pool_radius[l]); upsamples[l] = search(points_l, points_{l+1}, up_radius[l]). Every index matrix has exactly
  * limit[l] columns (nearest first, padded with the number of supports). Output buffers are caller-allocated with
- * `capacity[l]` rows per level.
+ * `capacity[l]` rows per level. Level-0 rows at or past the end of the last cloud (N0 > sum of lengths) belong to
+ * no cloud: they are not subsampled, no search returns them, and their neighbour and upsample rows are all padding.
  *   Exact form (out_level_sizes != NULL, a HOST int[n_levels]): receives the actual row counts; the call synchronises
  *   the stream once per subsampled level (the next level's launch sizes depend on the cell count) -- what the TF ops
  *   do (their output shapes are data dependent, tf_batch_subsampling.cpp:99-104).
  *   Static form (out_level_sizes == NULL): no device->host read at all. Launches are sized by capacity[l], every
  *   kernel reads its row count from d_counts[l] (DEVICE int[n_levels], written by this call), conditions that the exact
- *   form reports as errors are OR-ed into *d_status (DEVICE int: bit 0 = points outside host_bbox, bit 1 = a level
- *   has more cells than capacity[l+1]). The launch sequence depends only on (B, capacity, spec, host_bbox), so a
+ *   form reports as errors are OR-ed into *d_status (DEVICE int: bit 0 = a cloud whose extent needs more subsampling
+ *   cells than host_bbox allows, so its sort key overflows; bit 1 = a level has more cells than capacity[l+1]). A
+ *   cloud that is only displaced outside host_bbox sets no bit: its cells are keyed from its own origin and the
+ *   neighbour grids clamp it into their edge cells, so its pyramid is still exact. The launch sequence depends only on (B, capacity, spec, host_bbox), so a
  *   caller may capture it in a CUDA graph and replay it for every batch of the same bucket. d_counts[0] = N0, or
  *   *n0_dev when n0_dev != NULL (the level-0 count kept on the device; N0 is then the capacity of `points`).
  *   d_counts / d_status may be NULL in the exact form.

@@ -58,6 +58,40 @@ def test_invalid_arguments_return_codes_without_a_gpu(built_lib):
                                                           None) == 0
 
 
+@pytest.mark.parametrize("B", [0, 1025])
+def test_batch_size_checked_before_any_cuda_call(built_lib, B):
+    """Grid subsampling, the radius-neighbour build / count / fill and the pyramid take 1 to 1024 clouds; any other
+    number is refused before a kernel or a CUDA call (the pointers are never dereferenced)."""
+    from d3feat_b200._lib import SYMBOLS
+    lib = built_lib
+    lib.d3f_last_error.restype = ctypes.c_char_p
+    names = ("d3f_grid_subsample", "d3f_radius_neighbors_build", "d3f_radius_neighbors_count",
+             "d3f_radius_neighbors_fill", "d3f_pyramid_build")
+    for name in names:
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = [(r, a) for n, r, a in SYMBOLS if n == name][0]
+    fake = ctypes.c_void_p(256)
+    bbox = (ctypes.c_float * 6)(0, 0, 0, 1, 1, 1)
+    ptrs = (ctypes.c_void_p * 8)()
+    caps = (ctypes.c_int * 8)(*([100] * 8))
+    calls = {
+        "d3f_grid_subsample": lambda: lib.d3f_grid_subsample(fake, fake, B, 100, 0.1, None, 0, None, 0, bbox, fake, None,
+                                                             None, fake, fake, fake, 1 << 30, None),
+        "d3f_radius_neighbors_build": lambda: lib.d3f_radius_neighbors_build(fake, fake, B, 100, 0.1, bbox, fake, 1 << 30,
+                                                                             None),
+        "d3f_radius_neighbors_count": lambda: lib.d3f_radius_neighbors_count(fake, fake, 100, fake, fake, B, 100, 0.1,
+                                                                             bbox, fake, fake, fake, None),
+        # zero columns: nothing to write, but the batch size is still checked
+        "d3f_radius_neighbors_fill": lambda: lib.d3f_radius_neighbors_fill(fake, fake, 100, fake, fake, B, 100, 0.1, bbox,
+                                                                           fake, 0, 100, fake, None),
+        "d3f_pyramid_build": lambda: lib.d3f_pyramid_build(fake, fake, B, 100, fake, bbox, ptrs, ptrs, ptrs, ptrs, ptrs,
+                                                           caps, None, fake, 1 << 30, None, fake, fake, None),
+    }
+    for name in names:
+        assert calls[name]() == -1, name
+        assert (b"B=%d" % B) in lib.d3f_last_error(), (name, lib.d3f_last_error())
+
+
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):
     from d3feat_b200 import _lib
     monkeypatch.setattr(_lib, "_lib", None)

@@ -1,6 +1,8 @@
 """The element-wise check (tests/_oracle.py) is tight enough to matter: it rejects numpy emulations of the ways a KPConv,
 GEMM or detection-score kernel typically goes wrong, at the shapes of the GPU tests, and accepts the float32 evaluation
-of the same restatement (what an honest fp32 kernel with another summation order computes). No GPU needed."""
+of the same restatement (what an honest fp32 kernel with another summation order computes). The many-cloud batches of
+the subsampling and neighbour tests change the oracle's result under every emulated batch-assignment bug. No GPU
+needed."""
 import numpy as np
 import pytest
 
@@ -258,3 +260,72 @@ def test_detection_score_emulation_accepted_on_every_gpu_case(case):
     x, nbr, lengths = score_case(sum(map(ord, case)), lengths, D, H)
     ref, mag, alt = ok.detection_scores(f64(x), nbr, lengths, magnitude=True)
     assert_close(_emulated_scores(x, nbr, lengths), ref, mag, TOL / 10, "fp32 kernel emulation " + case, alt=alt)
+
+
+# ---- batch assignment: grid subsampling and radius neighbours of many clouds ----------------------------------------
+
+def _differs(a, b):
+    return a.shape != b.shape or not np.array_equal(a, b)
+
+
+def _first_row_to_previous_cloud(L):
+    """Lengths as a search that assigns the first row of every cloud to the previous non-empty cloud sees them."""
+    L = L.copy()
+    prev = None
+    for b in range(len(L)):
+        if L[b] > 0:
+            if prev is not None:
+                L[prev] += 1
+                L[b] -= 1
+            prev = b
+    return L
+
+
+def _empty_cloud_takes_next_row(L):
+    """Lengths as a search that gives an empty cloud the first row of the next cloud sees them."""
+    L = L.copy()
+    for b in range(len(L) - 1):
+        if L[b] == 0 and L[b + 1] > 0:
+            L[b], L[b + 1] = 1, L[b + 1] - 1
+    return L
+
+
+def _supports_of_the_neighbouring_cloud(q, qb, s, sb, r):
+    """Each query searched among the supports of the next cloud (the previous one for the last cloud)."""
+    from oracle import native as on
+    qs, ss = np.concatenate([[0], np.cumsum(qb)]), np.concatenate([[0], np.cumsum(sb)])
+    rows = []
+    for b in range(len(qb)):
+        o = b + 1 if b + 1 < len(qb) else b - 1
+        nb = on.port_batch_neighbors(q[qs[b]:qs[b + 1]], s[ss[o]:ss[o + 1]], [qb[b]], [sb[o]], r, pad_value=-1)
+        rows.append(np.where(nb >= 0, nb + ss[o], len(s)))
+    width = max(x.shape[1] for x in rows)
+    return np.concatenate([np.pad(x, ((0, 0), (0, width - x.shape[1])), constant_values=len(s)) for x in rows], 0)
+
+
+@pytest.mark.parametrize("case", ["B17", "B33", "B300", "B1024", "B1024_lone"])
+def test_many_cloud_batches_catch_batch_assignment_bugs(case):
+    """On the batches of tests/test_gpu_many_clouds.py, the oracle's result changes under each emulated way of putting a
+    row into the wrong cloud: the first row of every cloud in the previous non-empty cloud, an empty cloud taking the
+    next cloud's first row, the supports taken from the query's neighbouring cloud, and rows past the last cloud
+    joined to cloud B - 1."""
+    from test_gpu_many_clouds import DL, R, batch, oracle_neighbors, oracle_subsampling, search_args, tail_batch
+    P, L = batch(case)
+    ref_sub = oracle_subsampling(P, L, DL)
+    ref_nb = oracle_neighbors(P, L, P, L, R)[0]
+    bugs = {"first row in the previous cloud": _first_row_to_previous_cloud(L),
+            "empty cloud takes the next row": _empty_cloud_takes_next_row(L)}
+    for what, Lb in bugs.items():
+        if np.array_equal(Lb, L):
+            assert case.endswith("lone"), what          # no cloud to take a row from
+            continue
+        assert _differs(oracle_subsampling(P, Lb, DL)[0], ref_sub[0]), what
+        assert _differs(oracle_neighbors(P, Lb, P, Lb, R)[0], ref_nb), what
+    q, qb, s, sb, r = search_args(P, L, "pool")
+    assert _differs(_supports_of_the_neighbouring_cloud(q, qb, s, sb, r), oracle_neighbors(q, qb, s, sb, r)[0])
+    B = len(L)
+    P, L = tail_batch(B, -37)
+    Lb = L.copy()
+    Lb[-1] += 37                                            # the 37 rows of no cloud joined to cloud B - 1
+    assert _differs(oracle_subsampling(P, Lb, DL)[0], oracle_subsampling(P, L, DL)[0])
+    assert _differs(oracle_neighbors(P, Lb, P, Lb, R)[0], oracle_neighbors(P, L, P, L, R)[0])
