@@ -53,6 +53,8 @@ SYMBOLS = [
     ("d3f_register_pairs_workspace_bytes", _Z, [_I, _I, _I, _I]),
     ("d3f_register_pairs", _I, [_P, _P, _I, _I, _P, _P, _I, _P, _I, _I, _I, _I, _D, _D, _U64, _P, _P, _P, _P, _P, _Z,
                                 _P]),
+    ("d3f_icp_pairs_workspace_bytes", _Z, [_I, _I, _I, _D, _P]),
+    ("d3f_icp_pairs", _I, [_P, _P, _I, _I, _P, _P, _P, _I, _P, _D, _I, _D, _D, _P, _P, _P, _P, _P, _P, _Z, _P]),
 ]
 
 _lib = None

@@ -261,4 +261,17 @@ int d3f_register_pairs(const float* points, const int* count, int B, int k, cons
                         workspace_bytes, (cudaStream_t)stream);
 }
 
+size_t d3f_icp_pairs_workspace_bytes(int N, int B, int P, double distance, const float* host_bbox) {
+  return icp_pairs_workspace_bytes(N, B, P, distance, host_bbox);
+}
+
+int d3f_icp_pairs(const float* points, const int* lengths, int B, int N, const int* n_dev, const float* host_bbox,
+                  const int* pairs, int P, const double* init, double distance, int max_iterations,
+                  double relative_fitness, double relative_rmse, double* pose, double* fitness, double* inlier_rmse,
+                  int* n_corr, int* iterations, void* workspace, size_t workspace_bytes, d3f_stream_t stream) {
+  return icp_pairs(points, lengths, B, N, n_dev, host_bbox, pairs, P, init, distance, max_iterations,
+                   relative_fitness, relative_rmse, pose, fitness, inlier_rmse, n_corr, iterations, workspace,
+                   workspace_bytes, (cudaStream_t)stream);
+}
+
 }  // extern "C"

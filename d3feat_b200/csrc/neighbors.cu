@@ -7,43 +7,11 @@
 // r2 = radius*radius in fp32, rows ascending in (d2, index), padded with pad_value.
 #include <stdlib.h>
 
+#include "nbgrid.cuh"
 #include "ops.cuh"
 #include "sort.cuh"
 
 namespace d3f {
-
-struct NbGrid {
-  float minx, miny, minz, inv_cell;
-  int nx, ny, nz;
-  long long ncells;  // per cloud
-};
-
-static NbGrid make_grid(const float* host_bbox, float radius) {
-  NbGrid g;
-  float cell = radius * 1.001f;
-  g.inv_cell = 1.0f / cell;
-  g.minx = host_bbox[0];
-  g.miny = host_bbox[1];
-  g.minz = host_bbox[2];
-  auto dim = [&](int a) {
-    double ext = (double)host_bbox[3 + a] - (double)host_bbox[a];
-    if (!(ext >= 0)) ext = 0;
-    double n = floor(ext / (double)cell) + 2.0;
-    return n > 2.0e9 ? 2000000000 : (int)n;
-  };
-  g.nx = dim(0);
-  g.ny = dim(1);
-  g.nz = dim(2);
-  g.ncells = (long long)g.nx * g.ny * g.nz;
-  return g;
-}
-
-constexpr long long kMaxGridCells = 1ll << 27;  // 128 Mi cells total (2 x 4 B tables = 1 GiB)
-
-__device__ __forceinline__ int cell_coord(float v, float mn, float inv, int n) {
-  int c = (int)floorf((v - mn) * inv);
-  return min(max(c, 0), n - 1);
-}
 
 // Grid build = counting sort by cell: (1) count points per cell, (2) exclusive scan -> cell_start (cell c owns
 // [cell_start[c], cell_start[c+1])), (3) scatter. The order of the points INSIDE a cell is whatever the atomics give;
@@ -163,6 +131,22 @@ int radius_neighbors_order(const void* workspace, int Ns, int B, float radius, c
   carve_nb(cv, Ns, B, total, w);
   cell_order_kernel<<<ceil_div(Ns, 256), 256, 0, stream>>>(w.sorted_pts, Ns, out_order);
   D3F_LAUNCH_CHECK("cell_order_kernel");
+  return D3F_OK;
+}
+
+// The built grid of a workspace, for queries outside this file (nearest_in_cloud in nbgrid.cuh).
+int radius_neighbors_view(const void* workspace, int Ns, int B, float radius, const float* host_bbox, NbView* out) {
+  D3F_REQUIRE(B >= 1 && radius > 0.f && host_bbox != nullptr && out != nullptr, D3F_ERR_INVALID,
+              "radius_neighbors_view: bad arguments");
+  NbGrid g = make_grid(host_bbox, radius);
+  long long total = g.ncells * B;
+  D3F_REQUIRE(total <= kMaxGridCells, D3F_ERR_CAPACITY, "radius_neighbors: grid too large");
+  Carver cv(const_cast<void*>(workspace), ~(size_t)0);
+  NbWs w;
+  carve_nb(cv, Ns, B, total, w);
+  out->g = g;
+  out->sorted_pts = w.sorted_pts;
+  out->cell_start = w.cell_start;
   return D3F_OK;
 }
 

@@ -53,6 +53,8 @@ int radius_neighbors_fill(const float* queries, const int* q_batch_len, int Nq, 
                           const float* host_bbox, const void* workspace, int cols, int pad_value, int* out_idx,
                           cudaStream_t stream, const int* nq_dev = nullptr, const int* pad_dev = nullptr,
                           const int* q_start_pre = nullptr);
+struct NbView;   // nbgrid.cuh: the built grid, for nearest_in_cloud
+int radius_neighbors_view(const void* workspace, int Ns, int B, float radius, const float* host_bbox, NbView* out);
 
 // ---- pyramid.cu -------------------------------------------------------------------------------------
 size_t pyramid_workspace_bytes(int B, const d3f_pyramid_spec* spec, const int* capacity, const float* host_bbox);
@@ -113,5 +115,12 @@ int register_pairs(const float* points, const int* count, int B, int k, const in
                    const int* pairs, int P, int ransac_n, int max_iterations, int max_validation, double distance,
                    double edge_ratio, unsigned long long seed, double* pose, int* n_inliers, int* hypothesis,
                    int* n_validated, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+
+// ---- icp.cu -----------------------------------------------------------------------------------------
+size_t icp_pairs_workspace_bytes(int N, int B, int P, double distance, const float* host_bbox);
+int icp_pairs(const float* points, const int* lengths, int B, int N, const int* n_dev, const float* host_bbox,
+              const int* pairs, int P, const double* init, double distance, int max_iterations,
+              double relative_fitness, double relative_rmse, double* pose, double* fitness, double* inlier_rmse,
+              int* n_corr, int* iterations, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
 }  // namespace d3f

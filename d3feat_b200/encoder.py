@@ -16,7 +16,8 @@ from . import network_blocks as nb
 from . import pyramid
 from .keypoints import select_keypoints
 from .matching import host_pairs, match_keypoints
-from .registration import OPTIONS as REGISTER_OPTIONS, check_options, register_pairs
+from .registration import ICP_OPTIONS, OPTIONS as REGISTER_OPTIONS, check_icp_options, check_options, icp_pairs, \
+    register_pairs
 from .variables import ParamStore, use_params
 
 # GraphPipeline(..., keypoints=k) result: descriptors [cap0,32], scores [cap0,1], keypoints (KeypointSet, k per cloud)
@@ -25,6 +26,8 @@ Detections = namedtuple("Detections", "descriptors scores keypoints")
 MatchedDetections = namedtuple("MatchedDetections", "descriptors scores keypoints matches")
 # GraphPipeline(..., match_pairs=pairs, register={...}) result: the same plus registration (registration.Registration)
 RegisteredDetections = namedtuple("RegisteredDetections", "descriptors scores keypoints matches registration")
+# GraphPipeline(..., register={...}, icp={...}) result: the same plus refinement (registration.Refinement)
+RefinedDetections = namedtuple("RefinedDetections", "descriptors scores keypoints matches registration refinement")
 
 
 class KPFCNN:
@@ -223,12 +226,18 @@ class GraphPipeline:
 
     register={...} (needs match_pairs): the keyword arguments of registration.register_pairs ({} for the 3DMatch
     evaluation's defaults). The encoder graph then also estimates every pair's pose by RANSAC over its matches, and
-    `res` is a RegisteredDetections(descriptors, scores, keypoints, matches, registration)."""
+    `res` is a RegisteredDetections(descriptors, scores, keypoints, matches, registration).
+
+    icp=dict(distance=...) (needs register): the keyword arguments of registration.icp_pairs (distance,
+    max_iterations, relative_fitness, relative_rmse). The encoder graph then also refines every pair's RANSAC pose by
+    point-to-point ICP over the level-0 clouds of the batch (its points, lengths and device row count, within the
+    pipeline's bbox), and `res` is a RefinedDetections(descriptors, scores, keypoints, matches, registration,
+    refinement)."""
 
     DEPTH = 4
 
     def __init__(self, enc, capacities, n_clouds, bbox, decoder=False, post=None, encoder_streams=2, keypoints=None,
-                 match_pairs=None, register=None):
+                 match_pairs=None, register=None, icp=None):
         if keypoints is not None and not decoder:
             raise ValueError("GraphPipeline: keypoints=%r needs decoder=True (the detection scores)" % (keypoints,))
         if keypoints is not None and int(keypoints) < 1:
@@ -242,6 +251,14 @@ class GraphPipeline:
                 raise ValueError("GraphPipeline: register must be a dict of register_pairs options %s, got %r" % (
                     REGISTER_OPTIONS, register))
             check_options(**register, who="GraphPipeline")
+        if icp is not None:
+            if register is None:
+                raise ValueError("GraphPipeline: icp needs register (the RANSAC poses it refines)")
+            if not isinstance(icp, dict) or set(icp) - set(ICP_OPTIONS) or "distance" not in icp:
+                raise ValueError("GraphPipeline: icp must be a dict of icp_pairs options %s with a distance, got %r" % (
+                    ICP_OPTIONS, icp))
+            check_icp_options(**icp, who="GraphPipeline")
+        self.icp = None if icp is None else dict(icp)
         pairs = None if match_pairs is None else host_pairs(match_pairs, int(n_clouds), "GraphPipeline")
         self.register = None if register is None else dict(register)
         self.keypoints = None if keypoints is None else int(keypoints)
@@ -296,6 +313,10 @@ class GraphPipeline:
                 m = match_keypoints(kp, self.match_pairs)
                 if self.register is not None:
                     reg = register_pairs(kp, m, self.match_pairs, **self.register)
+                    if self.icp is not None:
+                        ref = icp_pairs(inputs["points"][0], inputs["lengths"][0], self.match_pairs, reg.pose,
+                                        rows=inputs["rows"][0], bbox=self.bbox, **self.icp)
+                        return F, RefinedDetections(desc, scores, kp, m, reg, ref)
                     return F, RegisteredDetections(desc, scores, kp, m, reg)
                 return F, MatchedDetections(desc, scores, kp, m)
             return F, Detections(desc, scores, kp)

@@ -11,10 +11,14 @@ Hypothesis h of pair p draws its sample from a counter-based splitmix64 of (seed
 on how the work is spread over the GPU. The parameters and checkers mean what Open3D's do; Open3D's own random
 sequence cannot be reproduced, so its poses are not reproduced bit for bit. The reference writes inv(pose) to its log
 (geometric_registration/evaluate.py:103-104); `pose` here maps source points onto the target, t' ~ R s + t.
+
+icp_pairs refines poses by point-to-point ICP over the dense clouds (d3f_icp_pairs), as the KITTI loader does with
+Open3D's registration_icp (datasets/KITTI.py:284-301); oracle/icp_np.py is its contract, exact in the same way.
 """
 import math
 from collections import namedtuple
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -28,6 +32,14 @@ Registration.__doc__ = """Registration of P cloud pairs. pose [P,4,4] float64 (t
     (validated hypotheses scored, at most max_validation)."""
 
 OPTIONS = ("distance", "ransac_n", "edge_ratio", "max_iterations", "max_validation", "seed", "mutual")
+
+Refinement = namedtuple("Refinement", "pose fitness inlier_rmse n_correspondences iterations")
+Refinement.__doc__ = """ICP refinement of P cloud pairs, all for the final pose. pose [P,4,4] float64 (t' ~ R s + t; row 3
+    copied from init), fitness [P] float64 (corresponding source rows / source rows), inlier_rmse [P] float64 (root mean
+    square distance of the correspondences, 0 without any), n_correspondences [P] int32, iterations [P] int32 (pose
+    updates made). A pair naming a cloud outside [0, B) or with an empty cloud keeps init with 0 everywhere."""
+
+ICP_OPTIONS = ("distance", "max_iterations", "relative_fitness", "relative_rmse")
 
 
 def check_options(distance=0.05, ransac_n=3, edge_ratio=0.9, max_iterations=50000, max_validation=1000, seed=0,
@@ -110,3 +122,81 @@ def register_pairs(kp, matches, pairs, *, distance=0.05, ransac_n=3, edge_ratio=
                                       _lib.stream()),
                "d3f_register_pairs")
     return Registration(pose, n_inliers, n_corr, hypothesis, n_validated)
+
+
+def check_icp_options(distance=None, max_iterations=30, relative_fitness=1e-6, relative_rmse=1e-6, who="icp_pairs"):
+    """The ICP options as (distance, max_iterations, relative_fitness, relative_rmse), each checked against the limits
+    of d3f_icp_pairs (ValueError). The defaults are Open3D's ICPConvergenceCriteria; distance has none."""
+    if isinstance(max_iterations, bool) or not isinstance(max_iterations, int) or not 0 <= max_iterations <= 1024:
+        raise ValueError("%s: max_iterations=%r must be an integer in [0, 1024]" % (who, max_iterations))
+    try:
+        tau, rf, rr = float(distance), float(relative_fitness), float(relative_rmse)
+    except (TypeError, ValueError):
+        raise ValueError("%s: distance=%r, relative_fitness=%r and relative_rmse=%r must be numbers" % (
+            who, distance, relative_fitness, relative_rmse))
+    if not (math.isfinite(tau) and tau > 0):
+        raise ValueError("%s: distance=%r must be finite and > 0" % (who, distance))
+    for name, v in (("relative_fitness", rf), ("relative_rmse", rr)):
+        if not (math.isfinite(v) and v >= 0):
+            raise ValueError("%s: %s=%r must be finite and >= 0" % (who, name, v))
+    return tau, max_iterations, rf, rr
+
+
+def icp_pairs(points, lengths, pairs, init=None, *, distance, max_iterations=30, relative_fitness=1e-6,
+              relative_rmse=1e-6, rows=None, bbox=None):
+    """Point-to-point ICP of every pair over stacked clouds, from `init`.
+
+    points: CUDA float32 [N,3], lengths [B] (cloud b holds rows [start[b], start[b+1]) of their exclusive scan; rows
+    past the last cloud belong to none). pairs: [P,2] (source cloud, target cloud); a host list or array is
+    range-checked against B (ValueError), a CUDA tensor is passed as it is, and a pair naming a cloud outside [0, B)
+    then keeps init. init: [P,4,4] float64 source-to-target poses (host or CUDA), the identity when None. rows: a
+    device int32 row count (N is then a capacity) or None. bbox: 6 floats bounding the clouds, the bounds of all N
+    rows when None (one device->host read); it only sizes the target grid (cell distance * 1.001), whose every
+    coordinate must lie within 1024 cells of the origin. The defaults are Open3D's ICPConvergenceCriteria; the KITTI
+    ground-truth refinement is icp_pairs(scans, lens, [(0, 1)], M, distance=0.2, max_iterations=200).
+    Returns Refinement(pose, fitness, inlier_rmse, n_correspondences, iterations)."""
+    tau, I, rf, rr = check_icp_options(distance, max_iterations, relative_fitness, relative_rmse)
+    if not torch.is_tensor(points) or not points.is_cuda or points.dtype != torch.float32 or points.dim() != 2 \
+            or int(points.shape[1]) != 3:
+        raise ValueError("icp_pairs: points must be a CUDA float32 tensor [N,3]")
+    points = points.contiguous()
+    dev = points.device
+    N = int(points.shape[0])
+    lens = _lib.i32(lengths, dev)
+    B = int(lens.numel())
+    if torch.is_tensor(pairs) and pairs.is_cuda:
+        if pairs.dim() != 2 or int(pairs.shape[1]) != 2:
+            raise ValueError("icp_pairs: pairs must be [P, 2], got %s" % (tuple(pairs.shape),))
+        pr = pairs.to(dtype=torch.int32).contiguous()
+    else:
+        pairs = pairs.numpy() if torch.is_tensor(pairs) else pairs
+        pr = torch.from_numpy(host_pairs(pairs, B, "icp_pairs")).to(dev)
+    P = int(pr.shape[0])
+    if init is None:
+        init = torch.eye(4, dtype=torch.float64, device=dev).expand(P, 4, 4)
+    init = torch.as_tensor(init).to(device=dev, dtype=torch.float64).contiguous()
+    if tuple(init.shape) != (P, 4, 4):
+        raise ValueError("icp_pairs: init must be [%d, 4, 4], got %s" % (P, tuple(init.shape)))
+    if rows is not None:
+        rows = _lib.i32(rows, dev).reshape(-1)[:1]
+    if bbox is None:
+        from .tf_custom_ops import host_bbox
+        bbox = host_bbox(points)
+    bbox = np.ascontiguousarray(bbox, np.float32).reshape(6)
+    lib = _lib.lib()
+    bb = bbox.ctypes.data_as(_lib.C.c_void_p)
+    nbytes = lib.d3f_icp_pairs_workspace_bytes(N, B, P, tau, bb)
+    if nbytes == 0:
+        raise ValueError("icp_pairs: no workspace for N=%d B=%d P=%d distance=%g bbox=%s: the grid exceeds its cell cap, "
+                         "a bbox coordinate lies beyond 1024 cells of the origin, or B is outside [1, 1024]" % (
+                             N, B, P, tau, bbox.tolist()))
+    ws = _lib.workspace(nbytes, dev)
+    pose = torch.empty((P, 4, 4), dtype=torch.float64, device=dev)
+    fitness, inlier_rmse = (torch.empty((P,), dtype=torch.float64, device=dev) for _ in range(2))
+    n_corr, iterations = (torch.empty((P,), dtype=torch.int32, device=dev) for _ in range(2))
+    _lib.check(lib.d3f_icp_pairs(_lib.ptr(points), _lib.ptr(lens), B, N, _lib.ptr(rows), bb, _lib.ptr(pr), P,
+                                 _lib.ptr(init), tau, I, rf, rr, _lib.ptr(pose), _lib.ptr(fitness),
+                                 _lib.ptr(inlier_rmse), _lib.ptr(n_corr), _lib.ptr(iterations), _lib.ptr(ws),
+                                 ws.numel(), _lib.stream()),
+               "d3f_icp_pairs")
+    return Refinement(pose, fitness, inlier_rmse, n_corr, iterations)

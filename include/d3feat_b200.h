@@ -31,6 +31,7 @@
  *   d3f_register_pairs        geometric_registration/evaluate.py:84-99, utils/tester.py:305-316,
  *                             demo_registration.py:184-192 (Open3D's RANSAC over the keypoint correspondences,
  *                             with the edge-length and distance checkers)
+ *   d3f_icp_pairs             datasets/KITTI.py:284-301 (Open3D's point-to-point registration_icp)
  */
 #ifndef D3FEAT_B200_H_
 #define D3FEAT_B200_H_
@@ -342,6 +343,38 @@ int d3f_register_pairs(const float* points, const int* count, int B, int k, cons
                        const int* pairs, int P, int ransac_n, int max_iterations, int max_validation, double distance,
                        double edge_ratio, unsigned long long seed, double* pose, int* n_inliers, int* hypothesis,
                        int* n_validated, void* workspace, size_t workspace_bytes, d3f_stream_t stream);
+
+/* Point-to-point ICP refinement of P cloud pairs over stacked clouds (datasets/KITTI.py:284-301, which calls
+ * Open3D's registration_icp with TransformationEstimationPointToPoint and ICPConvergenceCriteria).
+ *   points[N,3] fp32 and lengths[B] (device, >= 0) stacked as in d3f_radius_neighbors_build: cloud b holds the rows
+ *   [start[b], start[b+1]) of the lengths' exclusive scan, cut at the row count; rows at or past start[B] belong to no
+ *   cloud. n_dev (device, optional): the row count, N then being the capacity. host_bbox (host, 6 floats) sizes the
+ *   target grid as in the neighbour search; points outside it stay exact. pairs[P,2] (device) = (source cloud,
+ *   target cloud); init[P,4,4] (device, fp64, row-major) maps source points onto the target, t' ~ R s + t.
+ *   Contract (exact; oracle/icp_np.py restates it in numpy): every step is one correctly rounded fp64 operation in a
+ *   fixed order (no fused multiply-add), points widened from fp32 exactly. Evaluation i of pair p, pose T_i (T_0 =
+ *   init): every source row s becomes q = R s + t; its correspondence is the target row j with the smallest
+ *   d^2 = |q - t_j|^2 < distance^2 (strict; ties to the smaller row; NaN never corresponds). Over the n corresponding
+ *   rows, in blocks of 256 consecutive source rows summed sequentially and then the block sums sequentially: the
+ *   centroids, the centred cross-covariance and sum d^2. fitness = n / n_src, inlier_rmse = sqrt(sum d^2 / n) (0 for
+ *   n = 0). The pair stops after evaluation i > 0 when |fitness_i - fitness_{i-1}| < relative_fitness and
+ *   |rmse_i - rmse_{i-1}| < relative_rmse, when n < 3 (the pose is kept) or when i = max_iterations; otherwise
+ *   T_{i+1} = U T_i with U Horn's quaternion pose of (q, t_j) (6 cyclic Jacobi sweeps, as d3f_register_pairs).
+ *   Outputs, all for the final pose: pose[P,4,4] fp64 (rows 0-2 from T, row 3 copied from init), fitness[P],
+ *   inlier_rmse[P] (fp64), n_corr[P] and iterations[P] (the number of updates). A pair naming a cloud outside [0, B),
+ *   or with an empty source or target, keeps init with 0 correspondences and 0 iterations, and neither cloud is read.
+ *   Limits: B in [1, 1024]; N >= 0; P >= 1; max_iterations in [0, 1024]; distance finite and > 0; relative_fitness
+ *   and relative_rmse finite and >= 0; P * ceil(N / 256) * 256 within int32; the target grid (cell edge
+ *   distance * 1.001) within 2^27 cells over all clouds, and every host_bbox coordinate within 1024 cells of the origin
+ *   (the fp32 cell lookup of an fp64 query is then provably conservative). Otherwise, or for a null pointer (n_dev
+ *   excepted), D3F_ERR_INVALID before any CUDA call; D3F_ERR_WORKSPACE for a short workspace; the workspace query
+ *   returns 0 for arguments outside these limits. Graph-capturable: counts, pair ids and the stopping rule are
+ *   evaluated on the device; a call is 3 * max_iterations + 10 graph nodes (4 for N = 0). */
+size_t d3f_icp_pairs_workspace_bytes(int N, int B, int P, double distance, const float* host_bbox);
+int d3f_icp_pairs(const float* points, const int* lengths, int B, int N, const int* n_dev, const float* host_bbox,
+                  const int* pairs, int P, const double* init, double distance, int max_iterations,
+                  double relative_fitness, double relative_rmse, double* pose, double* fitness, double* inlier_rmse,
+                  int* n_corr, int* iterations, void* workspace, size_t workspace_bytes, d3f_stream_t stream);
 
 #ifdef __cplusplus
 }
