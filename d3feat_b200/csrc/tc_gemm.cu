@@ -11,8 +11,10 @@
 // * Two consumer warpgroups (M = 64 rows each, N = BN, K = 8 per instruction) read their A fragments from the swizzled
 //   stage with conflict-free 32-bit shared loads, split them into (hi, lo) in registers and issue the register-A (RS)
 //   form of wgmma against the B images in shared memory.
-// * Epilogue: each consumer thread applies rowscale / BN / bias / residual / LeakyReLU to its accumulator registers
-//   and stores them straight to global memory.
+// * Epilogue: each consumer warp turns its 16 x BN accumulator block through a 1 KB corner of shared memory, 8 rows x
+//   32 columns at a time, so that 8 lanes hold one row's 128 contiguous bytes. Rowscale / BN / bias / residual /
+//   LeakyReLU are applied in that layout (BN and bias vectors staged in shared memory once per column tile), and C and
+//   the residual move as whole 128-byte row pieces: 16-byte accesses when N % 4 == 0, single floats otherwise.
 // * Footprint: 9 warps; for BN <= 64 a CTA stays within half an SM's registers and shared memory, so two GEMM CTAs,
 //   or one GEMM CTA and the kernels of another stream, share an SM and cover each other's k-chunk drains and epilogues.
 #include <cuda.h>
@@ -79,7 +81,9 @@ int tc_pack_weight(const float* W, int K, int N, float* packed, cudaStream_t str
 //
 // Ring: a stage is one raw A chunk (16 KB) + the B hi/lo images. BN <= 64: two CTAs per SM, so <= 96 registers per
 // thread (9 warps per CTA: one of the SM's four register-file quarters holds 5 of the 18 warps) and <= 113 KB of shared
-// memory each; BN = 128 (64-register accumulators) keeps one CTA per SM and 3 stages.
+// memory each; BN = 128 (64-register accumulators) keeps one CTA per SM and 3 stages. The epilogue area (per consumer
+// warp one 1 KB pass and 3 x BN floats of column vectors) comes on top of the ring: 108 / 111 / 165 KB in all for
+// BN = 32 / 64 / 128.
 template <int BN>
 struct TcSmem {
   static constexpr int kCtasPerSm = BN >= 128 ? 1 : 2;
@@ -87,7 +91,8 @@ struct TcSmem {
   static constexpr int kABytes = kTcBM * 128;  // the raw fp32 A tile of one k-chunk
   static constexpr int kBBytes = BN * 128;     // one image (hi or lo) of the B tile
   static constexpr int kStageBytes = kABytes + 2 * kBBytes;
-  static constexpr int kTotal = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int kEpiWarpBytes = 1024 + 3 * BN * 4;  // per consumer warp: one epilogue pass + the column vectors
+  static constexpr int kTotal = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/ + kTcConsumerWarps * kEpiWarpBytes;
   static_assert(kCtasPerSm * (kTotal + 1024) <= 233472, "shared memory of an H100 SM (228 KB, 1 KB reserved per CTA)");
 };
 
@@ -121,7 +126,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   // split-K: CTA z owns the k-chunks [kt0, kt0 + nk) and writes raw partial sums to its own [M,N] slab of C
   const int kt0 = blockIdx.z * chunks_per_split;
   const int nk = min(Kpad / kTcBK - kt0, chunks_per_split);
-  C += (size_t)blockIdx.z * Mcap * N;
+  float* Cz = C + (size_t)blockIdx.z * Mcap * N;
 
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) {
@@ -177,9 +182,6 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int q = 0; q < 4; ++q)
         x[q] = lds32(sa + a_row + (uint32_t)(q & 1) * 1024u + ((((uint32_t)(2 * j + (q >> 1))) ^ a_swz) << 4));
     };
-    const bool has_bn = ep.bn_scale != nullptr, has_bias = ep.bias != nullptr, has_res = ep.residual != nullptr;
-    const bool has_leaky = ep.leaky_alpha >= 0.f;
-    const bool pairs = (N & 1) == 0;          // two adjacent columns of a row are one aligned 8-byte access
     float acc[R], sum[R];
     int g = 0;
     for (int t = (int)blockIdx.x; t < tiles; t += (int)gridDim.x) {
@@ -225,50 +227,97 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
         for (int j = 0; j < R; ++j) sum[j] += acc[j];
       }
-      // ===================== epilogue straight from the registers ===========================================
-      // A thread holds two rows (l/4 and l/4 + 8 of its warp's 16) x pairs of adjacent columns: the four lanes of a
-      // row cover 8 consecutive columns, i.e. every 32-byte sector a warp stores or loads (residual) is whole.
+      // ===================== epilogue: fragment -> shared memory -> whole 128-byte row pieces ======================
+      const bool has_bn = ep.bn_scale != nullptr, has_bias = ep.bias != nullptr, has_res = ep.residual != nullptr;
+      const bool has_leaky = ep.leaky_alpha >= 0.f;
+      // a lane's four adjacent columns of a row are one aligned 16-byte access (a split-K slab starts a multiple of
+      // N floats into C)
+      const bool vec = (N & 3) == 0 &&
+                       ((reinterpret_cast<uintptr_t>(C) | reinterpret_cast<uintptr_t>(ep.residual)) & 15) == 0;
+      // this warp's corner of the epilogue area: one 8 row x 128 B pass, then [bn_scale | bn_shift | bias] of BN columns
+      const uint32_t st_tile = smem_u32(smem + kStages * S::kStageBytes + 256) + (uint32_t)warp * S::kEpiWarpBytes;
+      const uint32_t st_par = st_tile + 1024u;
+      // The BN / bias vectors of this column tile, once per warp and again only when the tile's columns change.
+      if (t == (int)blockIdx.x || ntn > 1) {
+        for (int c = lane; c < BN; c += 32) {
+          const int n = n0 + c;
+          if (has_bn) {
+            sts32(st_par + 4u * c, n < N ? ep.bn_scale[n] : 0.f);
+            sts32(st_par + 4u * (BN + c), n < N ? ep.bn_shift[n] : 0.f);
+          }
+          if (has_bias) sts32(st_par + 4u * (2 * BN + c), n < N ? ep.bias[n] : 0.f);
+        }
+      }   // visible to the warp after the __syncwarp of the first pass below
+      // A pass moves 8 rows x 32 columns of the warp's 16 x BN block: the fragment layout (row l / 4, column pairs
+      // 8 j + 2 (l % 4)) goes in with 8-byte stores, and comes back as rows: 8 lanes hold the eight 16-byte pieces of
+      // one row, so a warp-wide access to C or the residual covers 4 rows x 128 contiguous bytes. Piece p of row r
+      // sits at p ^ (2 (r % 4)) ^ (r / 4): both the stores (half a warp = rows r..r + 3 x 2 pieces) and the loads (a
+      // quarter warp = one row) touch every bank once.
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int gm = m0 + 64 * cw + 16 * wq + (lane >> 2) + 8 * h;
-        if (gm >= M) continue;
-        const float rs = ep.rowscale != nullptr ? ep.rowscale[gm] : 1.f;
-        // output row: identity, or the caller's row map (KPConv walks its queries in the hash grid's cell order and
-        // scatters the rows back)
-        const size_t orow = ep.row_map ? (size_t)ep.row_map[gm] : (size_t)gm;
-        float* crow = C + orow * N;
-        const float* rrow = has_res ? ep.residual + orow * N : nullptr;
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int gn = n0 + 8 * j + 2 * (lane & 3);
-          if (gn >= N) continue;
-          const bool both = gn + 1 < N;
-          float y[2] = {sum[4 * j + 2 * h] * rs, sum[4 * j + 2 * h + 1] * rs};
-          float r[2] = {0.f, 0.f};
-          if (has_res) {
-            if (pairs && both) {
-              const float2 rv = *reinterpret_cast<const float2*>(rrow + gn);
-              r[0] = rv.x;
-              r[1] = rv.y;
-            } else {
-              r[0] = rrow[gn];
-              if (both) r[1] = rrow[gn + 1];
+        for (int cg = 0; cg < BN / 32; ++cg) {
+          {
+            const uint32_t r = (uint32_t)(lane >> 2), tq = (uint32_t)(lane & 3);
+            const uint32_t swz = ((r & 3u) << 1) ^ (r >> 2);
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = 4 * cg + jj;
+              sts64(st_tile + r * 128u + (((uint32_t)(2 * jj) + (tq >> 1)) ^ swz) * 16u + (tq & 1u) * 8u,
+                    sum[4 * j + 2 * h], sum[4 * j + 2 * h + 1]);
             }
           }
+          __syncwarp();
+          const int pc = lane & 7;                       // this lane's 16-byte piece: columns 4 pc .. 4 pc + 3
+          const int gn = n0 + 32 * cg + 4 * pc;
+          const uint32_t par = st_par + 4u * (32 * cg + 4 * pc);   // this lane's four columns of the vectors
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int n = both ? gn + e : gn;
-            if (has_bn) y[e] = fmaf(y[e], ep.bn_scale[n], ep.bn_shift[n]);
-            if (has_bias) y[e] += ep.bias[n];
-            y[e] += r[e];
-            if (has_leaky) y[e] = y[e] > 0.f ? y[e] : y[e] * ep.leaky_alpha;
+          for (int i = 0; i < 2; ++i) {
+            const uint32_t r = (uint32_t)(lane >> 3) + 4u * i;
+            const float4 v = lds128(st_tile + r * 128u + (((uint32_t)pc ^ ((r & 3u) << 1) ^ (r >> 2)) << 4));
+            const int gm = m0 + 64 * cw + 16 * wq + 8 * h + (int)r;
+            if (gm >= M || gn >= N) continue;
+            const float rs = ep.rowscale != nullptr ? ep.rowscale[gm] : 1.f;
+            // output row: identity, or the caller's row map (KPConv walks its queries in the hash grid's cell order
+            // and scatters the rows back)
+            const size_t orow = ep.row_map ? (size_t)ep.row_map[gm] : (size_t)gm;
+            float* cp = Cz + orow * N + gn;
+            const float* rp = has_res ? ep.residual + orow * N + gn : nullptr;
+            float y[4] = {v.x * rs, v.y * rs, v.z * rs, v.w * rs};
+            float res[4] = {0.f, 0.f, 0.f, 0.f};
+            if (has_res) {
+              if (vec) {
+                const float4 rv = *reinterpret_cast<const float4*>(rp);
+                res[0] = rv.x; res[1] = rv.y; res[2] = rv.z; res[3] = rv.w;
+              } else {
+#pragma unroll
+                for (int e = 0; e < 4; ++e)
+                  if (gn + e < N) res[e] = rp[e];
+              }
+            }
+            if (has_bn) {
+              const float4 sc = lds128(par), sh = lds128(par + 4u * BN);
+              y[0] = fmaf(y[0], sc.x, sh.x); y[1] = fmaf(y[1], sc.y, sh.y);
+              y[2] = fmaf(y[2], sc.z, sh.z); y[3] = fmaf(y[3], sc.w, sh.w);
+            }
+            if (has_bias) {
+              const float4 bi = lds128(par + 8u * BN);
+              y[0] += bi.x; y[1] += bi.y; y[2] += bi.z; y[3] += bi.w;
+            }
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              y[e] += res[e];
+              if (has_leaky) y[e] = y[e] > 0.f ? y[e] : y[e] * ep.leaky_alpha;
+            }
+            if (vec) {
+              *reinterpret_cast<float4*>(cp) = make_float4(y[0], y[1], y[2], y[3]);
+            } else {
+#pragma unroll
+              for (int e = 0; e < 4; ++e)
+                if (gn + e < N) cp[e] = y[e];
+            }
           }
-          if (pairs && both) {
-            *reinterpret_cast<float2*>(crow + gn) = make_float2(y[0], y[1]);
-          } else {
-            crow[gn] = y[0];
-            if (both) crow[gn + 1] = y[1];
-          }
+          __syncwarp();   // the pass has been read before the next one overwrites it
         }
       }
     }
