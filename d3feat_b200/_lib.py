@@ -55,6 +55,9 @@ SYMBOLS = [
                                 _P]),
     ("d3f_icp_pairs_workspace_bytes", _Z, [_I, _I, _I, _D, _P]),
     ("d3f_icp_pairs", _I, [_P, _P, _I, _I, _P, _P, _P, _I, _P, _D, _I, _D, _D, _P, _P, _P, _P, _P, _P, _Z, _P]),
+    ("d3f_evaluate_pairs_workspace_bytes", _Z, [_I, _I]),
+    ("d3f_evaluate_pairs", _I, [_P, _P, _I, _I, _P, _P, _I, _P, _I, _P, _P, _P, _P, _I, _P, _I, _D, _D, _D, _D, _D, _D,
+                                _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _Z, _P]),
 ]
 
 _lib = None

@@ -274,4 +274,20 @@ int d3f_icp_pairs(const float* points, const int* lengths, int B, int N, const i
                    workspace_bytes, (cudaStream_t)stream);
 }
 
+size_t d3f_evaluate_pairs_workspace_bytes(int P, int S) { return evaluate_pairs_workspace_bytes(P, S); }
+
+int d3f_evaluate_pairs(const float* points, const int* count, int B, int k, const int* matches, const int* n_matches,
+                       int L, const int* pairs, int P, const double* truth_pose, const double* truth_info,
+                       const int* truth_flags, const double* const* poses, int S, const int* levels, int R,
+                       double fmr_distance, double fmr_ratio, double repeat_distance, double err2, double rte_max,
+                       double rre_max_deg, int* valid, int* n_match_inliers, double* inlier_ratio, int* fmr_hit,
+                       int* n_repeated, double* repeatability, double* rte, double* rre_deg, double* rmse2,
+                       int* success, int* recall_hit, double* totals, void* workspace, size_t workspace_bytes,
+                       d3f_stream_t stream) {
+  return evaluate_pairs(points, count, B, k, matches, n_matches, L, pairs, P, truth_pose, truth_info, truth_flags,
+                        poses, S, levels, R, fmr_distance, fmr_ratio, repeat_distance, err2, rte_max, rre_max_deg,
+                        valid, n_match_inliers, inlier_ratio, fmr_hit, n_repeated, repeatability, rte, rre_deg, rmse2,
+                        success, recall_hit, totals, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
 }  // extern "C"

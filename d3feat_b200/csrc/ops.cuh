@@ -123,4 +123,14 @@ int icp_pairs(const float* points, const int* lengths, int B, int N, const int* 
               double relative_fitness, double relative_rmse, double* pose, double* fitness, double* inlier_rmse,
               int* n_corr, int* iterations, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
+// ---- evaluation.cu ----------------------------------------------------------------------------------
+size_t evaluate_pairs_workspace_bytes(int P, int S);
+int evaluate_pairs(const float* points, const int* count, int B, int k, const int* matches, const int* n_matches,
+                   int L, const int* pairs, int P, const double* truth_pose, const double* truth_info,
+                   const int* truth_flags, const double* const* poses, int S, const int* levels, int R,
+                   double fmr_distance, double fmr_ratio, double repeat_distance, double err2, double rte_max,
+                   double rre_max_deg, int* valid, int* n_match_inliers, double* inlier_ratio, int* fmr_hit,
+                   int* n_repeated, double* repeatability, double* rte, double* rre_deg, double* rmse2, int* success,
+                   int* recall_hit, double* totals, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+
 }  // namespace d3f

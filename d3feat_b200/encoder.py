@@ -14,6 +14,7 @@ import torch
 
 from . import network_blocks as nb
 from . import pyramid
+from .evaluation import OPTIONS as EVALUATE_OPTIONS, GroundTruth, check_evaluate_options, check_truth, evaluate_pairs
 from .keypoints import select_keypoints
 from .matching import host_pairs, match_keypoints
 from .registration import ICP_OPTIONS, OPTIONS as REGISTER_OPTIONS, check_icp_options, check_options, icp_pairs, \
@@ -28,6 +29,10 @@ MatchedDetections = namedtuple("MatchedDetections", "descriptors scores keypoint
 RegisteredDetections = namedtuple("RegisteredDetections", "descriptors scores keypoints matches registration")
 # GraphPipeline(..., register={...}, icp={...}) result: the same plus refinement (registration.Refinement)
 RefinedDetections = namedtuple("RefinedDetections", "descriptors scores keypoints matches registration refinement")
+# GraphPipeline(..., match_pairs=pairs, evaluate={...}) result: the same plus evaluation (evaluation.Evaluation);
+# registration / refinement are None when the pipeline does not run them
+EvaluatedDetections = namedtuple("EvaluatedDetections",
+                                 "descriptors scores keypoints matches registration refinement evaluation")
 
 
 class KPFCNN:
@@ -232,12 +237,21 @@ class GraphPipeline:
     max_iterations, relative_fitness, relative_rmse). The encoder graph then also refines every pair's RANSAC pose by
     point-to-point ICP over the level-0 clouds of the batch (its points, lengths and device row count, within the
     pipeline's bbox), and `res` is a RefinedDetections(descriptors, scores, keypoints, matches, registration,
-    refinement)."""
+    refinement).
+
+    evaluate={...} (needs match_pairs): the keyword arguments of evaluation.evaluate_pairs ({} for the 3DMatch
+    evaluation's defaults). Every batch then comes with its evaluation.GroundTruth of the match pairs, loaded into the
+    slot with its points: prime(points, lengths, truth=...), step(next_points, next_lengths, next_truth=...). The
+    encoder graph also scores the keypoints, the matches and, with register (and icp), the RANSAC (and ICP) poses
+    against it, and `res` is an EvaluatedDetections(descriptors, scores, keypoints, matches, registration, refinement,
+    evaluation) with that step's per-pair metrics and totals. step() adds the step's totals into a running fp64 vector
+    on the caller's stream, in step order; evaluation_totals() reads it (one device->host read, for
+    evaluation.summary(totals, pipe.evaluate_levels, pipe.evaluate_pose_sets)) and reset_evaluation() zeroes it."""
 
     DEPTH = 4
 
     def __init__(self, enc, capacities, n_clouds, bbox, decoder=False, post=None, encoder_streams=2, keypoints=None,
-                 match_pairs=None, register=None, icp=None):
+                 match_pairs=None, register=None, icp=None, evaluate=None):
         if keypoints is not None and not decoder:
             raise ValueError("GraphPipeline: keypoints=%r needs decoder=True (the detection scores)" % (keypoints,))
         if keypoints is not None and int(keypoints) < 1:
@@ -258,6 +272,15 @@ class GraphPipeline:
                 raise ValueError("GraphPipeline: icp must be a dict of icp_pairs options %s with a distance, got %r" % (
                     ICP_OPTIONS, icp))
             check_icp_options(**icp, who="GraphPipeline")
+        if evaluate is not None:
+            if match_pairs is None:
+                raise ValueError("GraphPipeline: evaluate needs match_pairs (the pairs it scores)")
+            if not isinstance(evaluate, dict) or set(evaluate) - set(EVALUATE_OPTIONS):
+                raise ValueError("GraphPipeline: evaluate must be a dict of evaluate_pairs options %s, got %r" % (
+                    EVALUATE_OPTIONS, evaluate))
+            self.evaluate_levels = check_evaluate_options(int(keypoints), **evaluate, who="GraphPipeline")[0]
+            self.evaluate_pose_sets = ("ransac",) * (register is not None) + ("icp",) * (icp is not None)
+        self.evaluate = None if evaluate is None else dict(evaluate)
         self.icp = None if icp is None else dict(icp)
         pairs = None if match_pairs is None else host_pairs(match_pairs, int(n_clouds), "GraphPipeline")
         self.register = None if register is None else dict(register)
@@ -286,6 +309,15 @@ class GraphPipeline:
         self.kernels_per_step = 0
         self.n_loaded = 0
         self.pending = None
+        if self.evaluate is not None:
+            P = int(self.match_pairs.shape[0])
+            f64 = torch.float64
+            # per slot: the batch's truth, loaded with its points (info always present; bit 1 cleared without one)
+            self.truth = [GroundTruth(torch.zeros((P, 4, 4), dtype=f64, device=dev),
+                                      torch.zeros((P, 6, 6), dtype=f64, device=dev),
+                                      torch.zeros((P,), dtype=torch.int32, device=dev)) for _ in range(self.DEPTH)]
+            n_tot = 4 + len(self.evaluate_levels) + 7 * len(self.evaluate_pose_sets)
+            self.eval_running = torch.zeros((n_tot,), dtype=f64, device=dev)
 
     @classmethod
     def for_batch(cls, enc, points, lengths, slack=1.125, margin=0.05, **kw):
@@ -303,7 +335,7 @@ class GraphPipeline:
     def _run_pyramid(self, k):
         return self.enc.build_inputs_static(self.slots[k])
 
-    def _run_encoder(self, inputs):
+    def _run_encoder(self, inputs, k):
         F = self.enc.encode(inputs)
         if self.keypoints is not None:
             desc, scores = self.enc.describe(inputs, F, with_scores=True)
@@ -311,6 +343,15 @@ class GraphPipeline:
                                   descriptors=desc, rows=inputs["rows"][0])
             if self.match_pairs is not None:
                 m = match_keypoints(kp, self.match_pairs)
+                if self.evaluate is not None:
+                    reg = ref = None
+                    if self.register is not None:
+                        reg = register_pairs(kp, m, self.match_pairs, **self.register)
+                        if self.icp is not None:
+                            ref = icp_pairs(inputs["points"][0], inputs["lengths"][0], self.match_pairs, reg.pose,
+                                            rows=inputs["rows"][0], bbox=self.bbox, **self.icp)
+                    ev = evaluate_pairs(kp, m, self.match_pairs, self.truth[k], reg, ref, **self.evaluate)
+                    return F, EvaluatedDetections(desc, scores, kp, m, reg, ref, ev)
                 if self.register is not None:
                     reg = register_pairs(kp, m, self.match_pairs, **self.register)
                     if self.icp is not None:
@@ -332,7 +373,7 @@ class GraphPipeline:
                 inputs = self._run_pyramid(k)
             self.s_enc.wait_stream(self.s_pyr)
             with torch.cuda.stream(self.s_enc):
-                self._run_encoder(inputs)
+                self._run_encoder(inputs, k)
             self.s_pyr.wait_stream(self.s_enc)
         torch.cuda.synchronize(self.enc.device)
         n0 = _lib.launch_count()
@@ -341,11 +382,18 @@ class GraphPipeline:
             inputs = self._run_pyramid(k)
         ge = torch.cuda.CUDAGraph()
         with torch.cuda.graph(ge, stream=self.s_enc):
-            F, res = self._run_encoder(inputs)
+            F, res = self._run_encoder(inputs, k)
         self.kernels_per_step = _lib.launch_count() - n0
         self.g_pyr[k], self.g_enc[k], self.out[k] = gp, ge, (inputs, F, res)
 
-    def _load(self, points, lengths, inputs_ready):
+    def _load(self, points, lengths, inputs_ready, truth=None):
+        if self.evaluate is not None and truth is None:
+            raise ValueError("GraphPipeline: evaluate needs the truth of every batch (prime(..., truth=...), "
+                             "step(..., next_truth=...))")
+        if self.evaluate is None and truth is not None:
+            raise ValueError("GraphPipeline: truth given to a pipeline built without evaluate")
+        if truth is not None:
+            check_truth(truth, int(self.match_pairs.shape[0]), "GraphPipeline")
         k = self.n_loaded % self.DEPTH
         self.n_loaded += 1
         if self.done[k] is not None:
@@ -366,22 +414,35 @@ class GraphPipeline:
             buf.points0[:n0].copy_(torch.as_tensor(points), non_blocking=True)
             buf.lengths0.copy_(torch.as_tensor(lengths), non_blocking=True)
             buf.n0.fill_(n0)
+            if truth is not None:
+                self._load_truth(k, truth)
             self.g_pyr[k].replay()
             self.ready[k].record(self.s_pyr)
-        for t in (points, lengths):
+        for t in [points, lengths] + ([] if truth is None else [x for x in truth if x is not None]):
             if torch.is_tensor(t) and t.is_cuda:
                 t.record_stream(self.s_pyr)
         return k
+
+    def _load_truth(self, k, truth):
+        """Copy a batch's truth into slot k (on the current stream); without info, flags bit 1 is cleared."""
+        dst = self.truth[k]
+        for d, x in ((dst.pose, truth.pose), (dst.flags, truth.flags)):
+            d.copy_(x if torch.is_tensor(x) else torch.from_numpy(np.ascontiguousarray(x)), non_blocking=True)
+        if truth.info is None:
+            dst.flags.bitwise_and_(1)
+        else:
+            x = truth.info
+            dst.info.copy_(x if torch.is_tensor(x) else torch.from_numpy(np.ascontiguousarray(x)), non_blocking=True)
 
     def _mark_inputs(self):
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream(self.enc.device))
         return ev
 
-    def prime(self, points, lengths):
-        self.pending = self._load(points, lengths, self._mark_inputs())
+    def prime(self, points, lengths, truth=None):
+        self.pending = self._load(points, lengths, self._mark_inputs(), truth)
 
-    def step(self, next_points=None, next_lengths=None, pre=None):
+    def step(self, next_points=None, next_lengths=None, pre=None, next_truth=None):
         """Replay encoder(current batch), then load + replay the pyramid of the next batch on the other stream.
         Returns (result buffer, device level counts) of the current batch, ordered on the caller's stream."""
         k = self.pending
@@ -402,8 +463,21 @@ class GraphPipeline:
             ev.record(s_enc)
             self.done[k] = ev
         cur.wait_event(ev)
-        self.pending = self._load(next_points, next_lengths, inputs_ready) if next_points is not None else None
+        if self.evaluate is not None:
+            # on the caller's stream, after this step's encoder: consecutive encoders may overlap on their two
+            # streams, so the running totals are never written inside a graph
+            self.eval_running.add_(self.out[k][2].evaluation.totals)
+        self.pending = (self._load(next_points, next_lengths, inputs_ready, next_truth)
+                        if next_points is not None else None)
         return res, self.slots[k].counts
+
+    def evaluation_totals(self):
+        """The running totals of every step since construction or reset_evaluation(), as float64 numpy (one
+        device->host read on the caller's stream): see evaluation.summary."""
+        return self.eval_running.cpu().numpy()
+
+    def reset_evaluation(self):
+        self.eval_running.zero_()
 
     def drain(self):
         self.s_pyr.synchronize()

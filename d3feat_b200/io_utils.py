@@ -7,6 +7,8 @@ clouds, and the per-fragment arrays the reference's offline evaluation consumes.
   * write_fragment   -- utils/tester.py:226-228: descriptors/<scene>/cloud_bin_N.D3Feat.npy,
                         keypoints/<scene>/cloud_bin_N.npy, scores/<scene>/cloud_bin_N.npy, the layout
                         geometric_registration/evaluate.py:39-50 reads back (get_keypts / get_desc / get_scores)
+  * load_log / load_info / truth_for_pairs -- a 3DMatch scene's gt.log / gt.info as evaluation.GroundTruth; gt.log
+                        holds target-to-source poses, the truth is their inverse, source to target
 """
 import os
 
@@ -113,3 +115,62 @@ def write_fragment(root, scene, num_frag, points, descriptors, scores, num_keypt
         np.save(p, arr.astype(np.float32))
         paths.append(p)
     return paths
+
+
+def _load_blocks(path, rows):
+    """Choi's trajectory format: blocks of a header line `i j n_frag` and `rows` lines of floats."""
+    with open(path) as fh:
+        lines = [ln.split() for ln in fh if ln.strip()]
+    if len(lines) % (rows + 1):
+        raise ValueError("%s: %d non-empty lines are not blocks of 1 + %d" % (path, len(lines), rows))
+    n = len(lines) // (rows + 1)
+    ids = np.zeros((n, 3), np.int64)
+    mats = np.zeros((n, rows, rows))
+    for b in range(n):
+        head = lines[b * (rows + 1)]
+        ids[b] = [int(x) for x in head[:3]]
+        mats[b] = [[float(x) for x in lines[b * (rows + 1) + 1 + r][:rows]] for r in range(rows)]
+    return ids, mats
+
+
+def load_log(path):
+    """(ids [M,3] int64 (i, j, n_frag), T [M,4,4] float64) of a gt.log (geometric_registration/utils.py:loadlog).
+    T maps fragment j onto fragment i (target to source): the reference transforms the target by it."""
+    return _load_blocks(path, 4)
+
+
+def load_info(path):
+    """(ids [M,3] int64 (i, j, n_frag), info [M,6,6] float64) of a gt.info: Choi's information matrices, read by
+    3dmatch/evaluate.m for mrEvaluateRegistration."""
+    return _load_blocks(path, 6)
+
+
+def counts_for_recall(i, j):
+    """Registration recall scores only non-consecutive fragments (mrEvaluateRegistration.m: j - i > 1)."""
+    return j - i > 1
+
+
+def truth_for_pairs(log, info, pairs):
+    """evaluation.GroundTruth of fragment pairs [(i, j), ...] (the cloud ids of a scene batch) from load_log's and
+    load_info's results (info may be None). A pair in the log gets flags bit 0 and G = inv(T_log), the source-to-target
+    pose (t ~ R s + t); it also gets bit 1 when j - i > 1 and info is given. Other pairs get flags 0 and the
+    identity."""
+    from .evaluation import GroundTruth
+    ids, T = log
+    pairs = np.asarray(pairs, np.int64).reshape(-1, 2)
+    P = pairs.shape[0]
+    at = {(int(i), int(j)): b for b, (i, j, _) in enumerate(ids)}
+    at_info = None if info is None else {(int(i), int(j)): b for b, (i, j, _) in enumerate(info[0])}
+    pose = np.tile(np.eye(4), (P, 1, 1))
+    inf = None if info is None else np.zeros((P, 6, 6))
+    flags = np.zeros(P, np.int32)
+    for p, (i, j) in enumerate(pairs.tolist()):
+        b = at.get((i, j))
+        if b is None:
+            continue
+        pose[p] = np.linalg.inv(T[b])
+        flags[p] = 1
+        if at_info is not None and (i, j) in at_info and counts_for_recall(i, j):
+            inf[p] = info[1][at_info[(i, j)]]
+            flags[p] |= 2
+    return GroundTruth(pose, inf, flags)

@@ -32,6 +32,9 @@
  *                             demo_registration.py:184-192 (Open3D's RANSAC over the keypoint correspondences,
  *                             with the edge-length and distance checkers)
  *   d3f_icp_pairs             datasets/KITTI.py:284-301 (Open3D's point-to-point registration_icp)
+ *   d3f_evaluate_pairs        geometric_registration/evaluate.py:67-82,207, repeatability/evaluate_3dmatch_our.py:30-41,
+ *                             evaluate_kitti_our.py:12-23, utils/tester.py:326-342, 3dmatch/evaluate.m with
+ *                             mrEvaluateRegistration.m (FMR, repeatability, RTE / RRE, registration recall)
  */
 #ifndef D3FEAT_B200_H_
 #define D3FEAT_B200_H_
@@ -375,6 +378,52 @@ int d3f_icp_pairs(const float* points, const int* lengths, int B, int N, const i
                   const int* pairs, int P, const double* init, double distance, int max_iterations,
                   double relative_fitness, double relative_rmse, double* pose, double* fitness, double* inlier_rmse,
                   int* n_corr, int* iterations, void* workspace, size_t workspace_bytes, d3f_stream_t stream);
+
+/* Ground-truth metrics of P matched and registered cloud pairs (geometric_registration/evaluate.py:67-82 and :207:
+ * feature-match recall; repeatability/evaluate_3dmatch_our.py:30-41, evaluate_kitti_our.py:12-23: repeatability;
+ * utils/tester.py:326-342: RTE / RRE / success; 3dmatch/evaluate.m with mrEvaluateRegistration.m: registration
+ * recall).
+ *   points[B,k,3] fp32 and count[B] (device) in the d3f_select_keypoints layout: cloud b's real slots are
+ *   [0, clamp(count[b], 0, k)) in ascending score, so its top n are the last n of them; no other slot is read.
+ *   matches[P,L,2] and n_matches[P] (device) as d3f_match_descriptors writes them. pairs[P,2] (device) = (source
+ *   cloud, target cloud). truth_pose[P,4,4] (device, fp64) maps source points onto the target (t ~ R s + t, the
+ *   convention of d3f_register_pairs; a 3DMatch gt.log holds the inverse). truth_info[P,6,6] (device, fp64, nullable):
+ *   Choi's information matrices. truth_flags[P] (device): bit 0 = the pair has truth, bit 1 = it counts for
+ *   registration recall. poses (host array of S device pointers, S in [0, 2]): [P,4,4] fp64 pose sets to score.
+ *   levels (host, R in [0, 14]): repeatability levels, strictly ascending within [1, k].
+ *   Contract (exact; oracle/evaluate_np.py restates it in numpy): every step is one correctly rounded fp64 operation
+ *   in a fixed order (no fused multiply-add), keypoints widened from fp32, q = R s + t in d3f_register_pairs' order,
+ *   every distance test d^2 < tau^2 (strict; the reference compares sqrt(d^2) < tau, which differs only at rounding
+ *   ties). A pair is evaluated when flags bit 0 is set and both cloud ids lie in [0, B):
+ *     n_match_inliers counts the rows m < clamp(n_matches, 0, L) whose real slots have d^2(G s_i, t_j) < fmr_distance^2;
+ *     inlier_ratio = n_match_inliers / n_matches (0 without matches); fmr_hit = inlier_ratio > fmr_ratio.
+ *     n_repeated[p,r] counts the target slots among the top levels[r] whose smallest d^2 over the top levels[r] source
+ *     slots is < repeat_distance^2 with no NaN d^2 among them; repeatability = n_repeated / levels[r].
+ *     Per pose set: rte = |t - t_G|; c = (tr(R^T R_G) - 1) / 2 clamped to [-1, 1]; rre_deg = acos(c) * 180 / pi
+ *     (acos is not correctly rounded: within a few ulp of the oracle); success = rte < rte_max and
+ *     c > cos(rre_max_deg). With flags bit 1 and truth_info: E = G inv(pose), er = [t_E; -q_v] (dcm2quat),
+ *     rmse2 = er^T info er / info_00, recall_hit = rmse2 <= err2 (NaN is a miss). A non-finite entry in rows 0-2 of G
+ *     or of the pose gives NaN rte, rre_deg and rmse2: a miss in every pose test.
+ *   Outputs (device, every element written): valid, n_match_inliers, fmr_hit [P] int32, inlier_ratio [P] fp64;
+ *   n_repeated [P,R] int32, repeatability [P,R] fp64; rte, rre_deg, rmse2 [S,P] fp64, success, recall_hit [S,P] int32
+ *   (NaN where undefined); totals [4 + R + 7 S] fp64, summed over the evaluated pairs sequentially in pair order:
+ *   pairs, FMR hits, sum inlier_ratio, sum n_match_inliers, sum repeatability per level, then per pose set:
+ *   successes, sum rte over rte < rte_max and that count, sum rre_deg over c > cos(rre_max_deg) and that count,
+ *   recall hits, recall pairs. A pair that is not evaluated reads nothing: valid 0, zeros, NaN rte / rre_deg / rmse2.
+ *   Limits: B in [1, 1024]; k, L, P >= 1; P*k, P*L*2 and B*k*3 within int32; fmr_distance, repeat_distance, err2 and
+ *   rte_max finite and > 0; fmr_ratio in [0, 1); rre_max_deg in (0, 180]. Otherwise, or for a null pointer
+ *   (truth_info excepted; the repeatability outputs when R = 0 and the pose outputs when S = 0),
+ *   D3F_ERR_INVALID before any CUDA call; D3F_ERR_WORKSPACE for a short workspace. Graph-capturable: counts, pair
+ *   ids, flags and truth are read on the device; a call is 2 to 4 kernels. */
+size_t d3f_evaluate_pairs_workspace_bytes(int P, int S);
+int d3f_evaluate_pairs(const float* points, const int* count, int B, int k, const int* matches, const int* n_matches,
+                       int L, const int* pairs, int P, const double* truth_pose, const double* truth_info,
+                       const int* truth_flags, const double* const* poses, int S, const int* levels, int R,
+                       double fmr_distance, double fmr_ratio, double repeat_distance, double err2, double rte_max,
+                       double rre_max_deg, int* valid, int* n_match_inliers, double* inlier_ratio, int* fmr_hit,
+                       int* n_repeated, double* repeatability, double* rte, double* rre_deg, double* rmse2,
+                       int* success, int* recall_hit, double* totals, void* workspace, size_t workspace_bytes,
+                       d3f_stream_t stream);
 
 #ifdef __cplusplus
 }
