@@ -104,6 +104,45 @@ def ptr(t):
     return C.c_void_p(t.data_ptr())
 
 
+DEVICE_TYPE = "cuda"     # where the kernels read their arguments
+
+
+def _describe(t):
+    if not torch.is_tensor(t):
+        return type(t).__name__
+    return "%s %s on %s" % (str(t.dtype).replace("torch.", ""), list(t.shape), t.device)
+
+
+def tensor_arg(t, name, dtype, shape=None, device=None, optional=False):
+    """The tensor argument `name` ("<op>: <argument>") of a hot-path op, contiguous, or ValueError: it must be a
+    `dtype` tensor on a CUDA device (`device`, when the call has already seen a tensor) whose shape matches `shape`,
+    a tuple with None for a free dimension. Nothing is converted: a silent .to(int32) here would be a hidden copy per
+    call, and a wrong dtype or a host address read by a kernel is a wrong result or a fault. Only attributes are read
+    (no launch, no synchronisation); .contiguous() copies a strided view and returns anything else as it is."""
+    if t is None and optional:
+        return None
+    ok = torch.is_tensor(t) and t.dtype == dtype
+    if ok:
+        dev = t.device
+        ok = dev.type == DEVICE_TYPE and (device is None or dev == device)
+    if ok and shape is not None:
+        got = t.shape
+        ok = len(got) == len(shape) and all(e is None or e == g for e, g in zip(shape, got))
+    if not ok:
+        want = "" if shape is None else " of shape [%s]" % ", ".join("*" if e is None else str(int(e)) for e in shape)
+        raise ValueError("%s must be a %s CUDA tensor%s%s, got %s" % (
+            name, str(dtype).replace("torch.", ""), want, "" if device is None else " on %s" % device, _describe(t)))
+    return t.contiguous()
+
+
+def row_count_arg(t, name, device):
+    """An optional device row count: one int32 element (tensor_arg otherwise)."""
+    t = tensor_arg(t, name, torch.int32, None, device, optional=True)
+    if t is not None and t.numel() != 1:
+        raise ValueError("%s must hold one int32 element, got %s" % (name, _describe(t)))
+    return t
+
+
 def workspace(nbytes, device):
     return torch.empty((max(int(nbytes), 256),), dtype=torch.uint8, device=device)
 

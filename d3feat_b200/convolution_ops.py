@@ -39,9 +39,12 @@ def packed_weight(w2d_view_of):
     w = w2d_view_of
     # keyed by the tensor OBJECT (weak): the entry dies with the tensor, so a recycled device address can never
     # alias a stale image; _version catches in-place updates
-    hit = _packed_cache.get(id(w))
+    hit = _packed_cache.get(id(w))           # (a hit was checked when it was packed)
     if hit is not None and hit[0]() is w and hit[1] == w._version:
         return hit[2]
+    w = _lib.tensor_arg(w, "packed_weight: weights", _F32)
+    if w.dim() < 2:
+        raise ValueError("packed_weight: weights must be [..., K, N], got %s" % (tuple(w.shape),))
     K = int(np.prod(w.shape[:-1]))
     N = int(w.shape[-1])
     L = _lib.lib()
@@ -53,32 +56,42 @@ def packed_weight(w2d_view_of):
     return packed
 
 
+_F32, _I32 = torch.float32, torch.int32
+
 _INFLUENCE = {"constant": 0, "linear": 1, "gaussian": 2}
 _MODE = {"sum": 0, "closest": 1}
 
 
-def _epilogue_args(epilogue):
+def _epilogue_args(epilogue, op, Cout, device):
     if epilogue is None:
         return None, None, -1.0
     scale, shift, alpha = epilogue
+    scale = _lib.tensor_arg(scale, op + ": epilogue scale", _F32, (Cout,), device)
+    shift = _lib.tensor_arg(shift, op + ": epilogue shift", _F32, (Cout,), device)
     return scale, shift, (-1.0 if alpha is None else float(alpha))
 
 
 def unary_convolution(features, K_values, *, epilogue=None, residual=None, rows=None):
     """features[N,Cin] @ K_values[Cin,Cout] (tf.matmul, :90-99).
     rows (extension): int32 device scalar holding the actual row count when `features` is a capacity-sized buffer."""
-    x = features.contiguous()
-    w = K_values.contiguous()
+    op = "unary_convolution"
+    x = _lib.tensor_arg(features, op + ": features", _F32, (None, None))
+    dev = x.device
     N, Cin = x.shape
+    w = _lib.tensor_arg(K_values, op + ": K_values", _F32, (Cin, None), dev)
     Cout = w.shape[1]
-    if w.shape[0] != Cin:
-        raise ValueError("unary_convolution: features %s do not match K_values %s" % (tuple(x.shape), tuple(w.shape)))
-    scale, shift, alpha = _epilogue_args(epilogue)
-    out = torch.empty((N, Cout), dtype=torch.float32, device=x.device)
+    scale, shift, alpha = _epilogue_args(epilogue, op, Cout, dev)
+    res = _lib.tensor_arg(residual, op + ": residual", _F32, (N, Cout), dev, optional=True)
+    rows = _lib.row_count_arg(rows, op + ": rows", dev)
+    out = torch.empty((N, Cout), dtype=torch.float32, device=dev)
     _lib.check(_lib.lib().d3f_unary_forward(_lib.ptr(x), _lib.ptr(w), _lib.ptr(packed_weight(w)), N, Cin, Cout, _lib.ptr(scale), _lib.ptr(shift),
-                                            None, _lib.ptr(residual.contiguous()) if residual is not None else None,
-                                            alpha, _lib.ptr(out), _lib.stream(), _lib.ptr(rows)), "d3f_unary_forward")
+                                            None, _lib.ptr(res), alpha, _lib.ptr(out), _lib.stream(), _lib.ptr(rows)),
+               "d3f_unary_forward")
     return out
+
+
+def _aligned16(t):
+    return t.data_ptr() % 16 == 0
 
 
 _pair_cache = {}       # (id(w1), id(w2)) -> (refs, versions, packed image of the folded [w1*s1 ; w2*s2], shift1 + shift2)
@@ -89,16 +102,22 @@ def unary_pair_convolution(x1, w1, affine1, x2, w2, affine2, alpha, *, rows=None
     + add + LeakyReLU tail of a resnetb block (models/network_blocks.py:343-368). affine = (scale, shift) of the
     unary's inference batch norm. The scales are folded into the weights once per weight pair (float64), so neither
     the shortcut tensor nor [x1 | x2] exists in memory. Falls back to two unary_convolution calls without the
-    tensor-core path or when the channel counts do not tile."""
-    x1, x2 = x1.contiguous(), x2.contiguous()
-    (s1, t1), (s2, t2) = affine1, affine2
+    tensor-core path, when the channel counts do not tile, or when x1 or x2 does not start on a 16-byte boundary (the
+    one-GEMM kernel fetches both by TMA; a lone unary_convolution then runs its CUDA-core GEMM on that operand)."""
+    op = "unary_pair_convolution"
+    x1 = _lib.tensor_arg(x1, op + ": x1", _F32, (None, None))
+    dev = x1.device
     N, C1 = x1.shape
+    x2 = _lib.tensor_arg(x2, op + ": x2", _F32, (N, None), dev)
     C2 = int(x2.shape[1])
+    w1 = _lib.tensor_arg(w1, op + ": w1", _F32, (C1, None), dev)
     Cout = int(w1.shape[1])
-    if w1.shape[0] != C1 or w2.shape[0] != C2 or w2.shape[1] != Cout or x2.shape[0] != N:
-        raise ValueError("unary_pair_convolution: shapes %s@%s + %s@%s" % (tuple(x1.shape), tuple(w1.shape),
-                                                                             tuple(x2.shape), tuple(w2.shape)))
-    if not USE_TENSOR_CORES or C1 % 32 != 0 or C2 % 4 != 0:
+    w2 = _lib.tensor_arg(w2, op + ": w2", _F32, (C2, Cout), dev)
+    (s1, t1), (s2, t2) = affine1, affine2
+    s1, t1, s2, t2 = (_lib.tensor_arg(v, "%s: affine%s" % (op, n), _F32, (Cout,), dev)
+                      for v, n in ((s1, "1 scale"), (t1, "1 shift"), (s2, "2 scale"), (t2, "2 shift")))
+    rows = _lib.row_count_arg(rows, op + ": rows", dev)
+    if not USE_TENSOR_CORES or C1 % 32 != 0 or C2 % 4 != 0 or not (_aligned16(x1) and _aligned16(x2)):
         shortcut = unary_convolution(x2, w2, epilogue=(s2, t2, None), rows=rows)
         return unary_convolution(x1, w1, epilogue=(s1, t1, alpha), residual=shortcut, rows=rows)
     key = (id(w1), id(w2))
@@ -129,6 +148,23 @@ def _check_enums(KP_influence, aggregation_mode):
         raise ValueError("Unknown convolution mode. Should be 'closest' or 'sum'")         # :232, :477
 
 
+def _kpconv_args(op, query_points, support_points, neighbors_indices, features, K_points, K_values, query_order,
+                 rows_q, rows_s):
+    """The tensor arguments both KPConv ops share, checked against each other (ValueError) and contiguous."""
+    q = _lib.tensor_arg(query_points, op + ": query_points", _F32, (None, 3))
+    dev = q.device
+    Nq = q.shape[0]
+    s = _lib.tensor_arg(support_points, op + ": support_points", _F32, (None, 3), dev)
+    Ns = s.shape[0]
+    idx = _lib.tensor_arg(neighbors_indices, op + ": neighbors_indices", _I32, (Nq, None), dev)
+    f = _lib.tensor_arg(features, op + ": features", _F32, (Ns, None), dev)
+    W = _lib.tensor_arg(K_values, op + ": K_values", _F32, (None, f.shape[1], None), dev)
+    Kp = _lib.tensor_arg(K_points, op + ": K_points", _F32, (W.shape[0], 3), dev)
+    order = _lib.tensor_arg(query_order, op + ": query_order", _I32, (Nq,), dev, optional=True)
+    return (q, s, idx, f, Kp, W, order, _lib.row_count_arg(rows_q, op + ": rows_q", dev),
+            _lib.row_count_arg(rows_s, op + ": rows_s", dev))
+
+
 def KPConv_ops(query_points, support_points, neighbors_indices, features, K_points, K_values, KP_extent,
                KP_influence, aggregation_mode, *, epilogue=None, bias=None, query_order=None, rows_q=None,
                rows_s=None):
@@ -138,15 +174,13 @@ def KPConv_ops(query_points, support_points, neighbors_indices, features, K_poin
     rows_q / rows_s (extension): int32 device scalars with the actual query / support counts when the tensors are
     capacity-sized buffers (the shadow index is then the actual support count)."""
     _check_enums(KP_influence, aggregation_mode)
-    q, s = query_points.contiguous(), support_points.contiguous()
-    idx, f = neighbors_indices.contiguous(), features.contiguous()
-    Kp, W = K_points.contiguous(), K_values.contiguous()
+    op = "KPConv_ops"
+    q, s, idx, f, Kp, W, query_order, rows_q, rows_s = _kpconv_args(
+        op, query_points, support_points, neighbors_indices, features, K_points, K_values, query_order, rows_q, rows_s)
     Nq, Ns, H = q.shape[0], s.shape[0], idx.shape[1]
     K, Cin, Cout = W.shape
-    if f.shape[0] != Ns or f.shape[1] != Cin or Kp.shape[0] != K or idx.shape[0] != Nq:
-        raise ValueError("KPConv_ops: inconsistent shapes q%s s%s idx%s f%s Kp%s W%s" % (
-            tuple(q.shape), tuple(s.shape), tuple(idx.shape), tuple(f.shape), tuple(Kp.shape), tuple(W.shape)))
-    scale, shift, alpha = _epilogue_args(epilogue)
+    scale, shift, alpha = _epilogue_args(epilogue, op, Cout, q.device)
+    bias = _lib.tensor_arg(bias, op + ": bias", _F32, (Cout,), q.device, optional=True)
     L = _lib.lib()
     ws = _lib.workspace(L.d3f_kpconv_workspace_bytes(Nq, Ns, H, K, Cin, Cout), q.device)
     out = torch.empty((Nq, Cout), dtype=torch.float32, device=q.device)
@@ -164,13 +198,14 @@ def KPConv_deform_ops(query_points, support_points, neighbors_indices, features,
                       rows_s=None):
     """Deformable second stage (:379-499)."""
     _check_enums(KP_influence, mode)
-    q, s = query_points.contiguous(), support_points.contiguous()
-    idx, f = neighbors_indices.contiguous(), features.contiguous()
-    Kp, W, off = K_points.contiguous(), K_values.contiguous(), offsets.contiguous()
-    mod = modulations.contiguous() if modulations is not None else None
+    op = "KPConv_deform_ops"
+    q, s, idx, f, Kp, W, query_order, rows_q, rows_s = _kpconv_args(
+        op, query_points, support_points, neighbors_indices, features, K_points, K_values, query_order, rows_q, rows_s)
     Nq, Ns, H = q.shape[0], s.shape[0], idx.shape[1]
     K, Cin, Cout = W.shape
-    scale, shift, alpha = _epilogue_args(epilogue)
+    off = _lib.tensor_arg(offsets, op + ": offsets", _F32, (Nq, K, 3), q.device)
+    mod = _lib.tensor_arg(modulations, op + ": modulations", _F32, (Nq, K), q.device, optional=True)
+    scale, shift, alpha = _epilogue_args(epilogue, op, Cout, q.device)
     L = _lib.lib()
     ws = _lib.workspace(L.d3f_kpconv_workspace_bytes(Nq, Ns, H, K, Cin, Cout), q.device)
     out = torch.empty((Nq, Cout), dtype=torch.float32, device=q.device)

@@ -57,9 +57,10 @@ struct Rows {
   int k, L;
   template <typename F>
   __device__ __forceinline__ void load(int p, int src, int tgt, int r, F s[3], F t[3]) const {
-    const int2 c = __ldg(reinterpret_cast<const int2*>(corr) + (size_t)p * L + r);
-    const float* ps = points + ((size_t)src * k + c.x) * 3;
-    const float* pt = points + ((size_t)tgt * k + c.y) * 3;
+    // two 4-byte loads: a caller's corr is only known to be int-aligned (a slice of a longer match buffer)
+    const int* c = corr + 2 * ((size_t)p * L + r);
+    const float* ps = points + ((size_t)src * k + __ldg(c)) * 3;
+    const float* pt = points + ((size_t)tgt * k + __ldg(c + 1)) * 3;
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
       s[i] = __ldg(ps + i);
@@ -142,8 +143,8 @@ reg_prepare_kernel(const int* __restrict__ count, int B, int k, const int* __res
     nc = min(max(__ldg(n_corr + p), 0), L);
     bool bad = false;
     for (int r = lane; r < nc; r += 32) {
-      const int2 c = __ldg(reinterpret_cast<const int2*>(corr) + (size_t)p * L + r);
-      bad = bad || c.x < 0 || c.x >= ns || c.y < 0 || c.y >= nt;
+      const int cs = __ldg(corr + 2 * ((size_t)p * L + r)), ct = __ldg(corr + 2 * ((size_t)p * L + r) + 1);
+      bad = bad || cs < 0 || cs >= ns || ct < 0 || ct >= nt;
     }
     if (__any_sync(0xffffffffu, bad)) nc = -1;
   }

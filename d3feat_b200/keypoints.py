@@ -31,19 +31,14 @@ def select_keypoints(scores, lengths, k=None, points=None, descriptors=None, *, 
     and `descriptors` [N,D] when given.
     rows: optional device int32 scalar with the actual row count (the static pyramid's level-0 count); N is then the
     capacity of the inputs and no row at or past it is read (order[rows:] is left unwritten)."""
-    s = scores.reshape(-1)
-    if not s.is_cuda or s.dtype != torch.float32:
-        raise ValueError("select_keypoints: scores must be a CUDA float32 tensor")
-    s = s.contiguous()
+    op = "select_keypoints"
+    s = _lib.tensor_arg(scores, op + ": scores", torch.float32).reshape(-1)
     dev = s.device
     lens = _lib.i32(lengths, dev)
     N, B = int(s.shape[0]), int(lens.shape[0])
-    pts = _lib.f32(points, dev) if points is not None else None
-    desc = _lib.f32(descriptors, dev) if descriptors is not None else None
-    if pts is not None and tuple(pts.shape) != (N, 3):
-        raise ValueError("select_keypoints: points %s do not match %d scores" % (tuple(pts.shape), N))
-    if desc is not None and (desc.dim() != 2 or int(desc.shape[0]) != N):
-        raise ValueError("select_keypoints: descriptors %s do not match %d scores" % (tuple(desc.shape), N))
+    pts = _lib.tensor_arg(points, op + ": points", torch.float32, (N, 3), dev, optional=True)
+    desc = _lib.tensor_arg(descriptors, op + ": descriptors", torch.float32, (N, None), dev, optional=True)
+    rows = _lib.row_count_arg(rows, op + ": rows", dev)
     D = int(desc.shape[1]) if desc is not None else 0
     lib = _lib.lib()
     ws = _lib.workspace(lib.d3f_select_keypoints_workspace_bytes(N, B), dev)

@@ -50,9 +50,19 @@ def _rows(inputs, level):
     return rows[level]
 
 
+_F32, _I32 = torch.float32, torch.int32
+
+
+def _pool_args(op, x, inds, rows_x, rows_out):
+    x = _lib.tensor_arg(x, op + ": x", _F32, (None, None))
+    inds = _lib.tensor_arg(inds, op + ": inds", _I32, (None, None), x.device)
+    return (x, inds, _lib.row_count_arg(rows_x, op + ": rows_x", x.device),
+            _lib.row_count_arg(rows_out, op + ": rows_out", x.device))
+
+
 def ind_max_pool(x, inds, *, rows_x=None, rows_out=None):
     """:51-66 -- max over the pooled rows; shadow index -> column-wise minimum of x."""
-    x, inds = x.contiguous(), inds.contiguous()
+    x, inds, rows_x, rows_out = _pool_args("ind_max_pool", x, inds, rows_x, rows_out)
     N1, C = x.shape
     N2, H = inds.shape
     L = _lib.lib()
@@ -65,7 +75,7 @@ def ind_max_pool(x, inds, *, rows_x=None, rows_out=None):
 
 def closest_pool(x, inds, *, rows_x=None, rows_out=None):
     """:69-83 -- features of the closest pooled point (first index column); shadow -> zeros."""
-    x, inds = x.contiguous(), inds.contiguous()
+    x, inds, rows_x, rows_out = _pool_args("closest_pool", x, inds, rows_x, rows_out)
     N1, C = x.shape
     N2, H = inds.shape
     out = torch.empty((N2, C), dtype=torch.float32, device=x.device)
@@ -75,11 +85,15 @@ def closest_pool(x, inds, *, rows_x=None, rows_out=None):
 
 
 def _affine_leaky(x, scale, shift, residual, alpha, rows=None):
-    x = x.contiguous()
+    op = "affine_leaky"
+    x = _lib.tensor_arg(x, op + ": x", _F32, (None, None))
     N, C = x.shape
+    scale = _lib.tensor_arg(scale, op + ": scale", _F32, (C,), x.device, optional=True)
+    shift = _lib.tensor_arg(shift, op + ": shift", _F32, (C,), x.device, optional=True)
+    residual = _lib.tensor_arg(residual, op + ": residual", _F32, (N, C), x.device, optional=True)
+    rows = _lib.row_count_arg(rows, op + ": rows", x.device)
     out = torch.empty_like(x)
-    _lib.check(_lib.lib().d3f_affine_leaky(_lib.ptr(x), N, C, _lib.ptr(scale), _lib.ptr(shift),
-                                           _lib.ptr(residual.contiguous()) if residual is not None else None,
+    _lib.check(_lib.lib().d3f_affine_leaky(_lib.ptr(x), N, C, _lib.ptr(scale), _lib.ptr(shift), _lib.ptr(residual),
                                            -1.0 if alpha is None else float(alpha), _lib.ptr(out), _lib.stream(),
                                            _lib.ptr(rows)), "d3f_affine_leaky")
     return out
@@ -292,9 +306,11 @@ def detection_scores(features, neighbors, lengths, *, rows=None):
     """Detection branch of models/D3Feat.py:67-115 on the decoder output BEFORE l2 normalisation: per-cloud max
     normalisation, softplus(x - mean over the non-zero neighbours), channel-max ratio, max over channels -> [N, 1].
     The reference hard-codes two clouds per batch (anchor || positive); here any number of stacked clouds."""
-    x = features.contiguous()
-    nbr = neighbors.contiguous()
-    lens = _lib.i32(lengths, x.device)
+    op = "detection_scores"
+    x = _lib.tensor_arg(features, op + ": features", _F32, (None, None))
+    nbr = _lib.tensor_arg(neighbors, op + ": neighbors", _I32, (x.shape[0], None), x.device)
+    lens = _lib.tensor_arg(lengths, op + ": lengths", _I32, (None,), x.device)
+    rows = _lib.row_count_arg(rows, op + ": rows", x.device)
     N, D = int(x.shape[0]), int(x.shape[1])
     B, H = int(lens.shape[0]), int(nbr.shape[1])
     out = torch.empty((N, 1), dtype=torch.float32, device=x.device)
@@ -303,6 +319,16 @@ def detection_scores(features, neighbors, lengths, *, rows=None):
     _lib.check(lib.d3f_detection_scores(_lib.ptr(x), _lib.ptr(nbr), _lib.ptr(lens), B, N, H, D, _lib.ptr(out),
                                         _lib.ptr(ws), ws.numel(), _lib.stream(), _lib.ptr(rows)),
                "d3f_detection_scores")
+    return out
+
+
+def l2_normalize(features, *, rows=None):
+    """models/D3Feat.py:65 -- x * rsqrt(max(sum x^2, 1e-10)) per row."""
+    x = _lib.tensor_arg(features, "l2_normalize: features", _F32, (None, None))
+    rows = _lib.row_count_arg(rows, "l2_normalize: rows", x.device)
+    out = torch.empty_like(x)
+    _lib.check(_lib.lib().d3f_l2_normalize(_lib.ptr(x), x.shape[0], x.shape[1], 1e-10, _lib.ptr(out), _lib.stream(),
+                                           _lib.ptr(rows)), "d3f_l2_normalize")
     return out
 
 
@@ -337,9 +363,7 @@ def assemble_FCNN_decoder(inputs, config, F, dropout_prob=1.0, with_scores=False
             fdim = fdim // 2
             block_in_layer = 0
             features = torch.cat((features, F[layer]), dim=1)
-    out = torch.empty_like(features)
-    _lib.check(_lib.lib().d3f_l2_normalize(_lib.ptr(features.contiguous()), features.shape[0], features.shape[1], 1e-10,
-                                           _lib.ptr(out), _lib.stream(), _lib.ptr(_rows(inputs, 0))), "d3f_l2_normalize")
+    out = l2_normalize(features, rows=_rows(inputs, 0))
     if with_scores:
         return out, detection_scores(features, inputs["neighbors"][0], inputs["lengths"][0], rows=_rows(inputs, 0))
     return out

@@ -25,7 +25,7 @@ from . import _lib
 
 def host_bbox(points):
     """float32[6] numpy bbox of a CUDA point tensor via the d3f_bbox kernel (one device->host read)."""
-    pts = points
+    pts = _lib.tensor_arg(points, "host_bbox: points", torch.float32, (None, 3))
     out = torch.empty((6,), dtype=torch.float32, device=pts.device)
     _lib.check(_lib.lib().d3f_bbox(_lib.ptr(pts), pts.shape[0], _lib.ptr(out), _lib.stream()), "d3f_bbox")
     bb = out.cpu().numpy().astype(np.float32)
@@ -47,8 +47,9 @@ class NeighborGrid:
     """Hash grid over the supports (d3f_radius_neighbors_build); reusable for several query sets."""
 
     def __init__(self, supports, s_batches, radius, bbox=None):
-        self.s = supports
-        self.sb = s_batches
+        self.s = _lib.tensor_arg(supports, "NeighborGrid: supports", torch.float32, (None, 3))
+        self.sb = _lib.tensor_arg(s_batches, "NeighborGrid: s_batches", torch.int32, (None,), self.s.device)
+        supports, s_batches = self.s, self.sb
         self.radius = float(radius)
         self.B = int(s_batches.shape[0])
         self.Ns = int(supports.shape[0])
@@ -71,7 +72,12 @@ class NeighborGrid:
                                                          _lib.ptr(out), _lib.stream()), "d3f_radius_neighbors_order")
         return out[:self.Ns]
 
+    def _queries(self, op, queries, q_batches):
+        q = _lib.tensor_arg(queries, "NeighborGrid.%s: queries" % op, torch.float32, (None, 3), self.s.device)
+        return q, _lib.tensor_arg(q_batches, "NeighborGrid.%s: q_batches" % op, torch.int32, (self.B,), self.s.device)
+
     def count(self, queries, q_batches):
+        queries, q_batches = self._queries("count", queries, q_batches)
         Nq = int(queries.shape[0])
         counts = torch.empty((max(Nq, 1),), dtype=torch.int32, device=queries.device)
         mx = torch.zeros((1,), dtype=torch.int32, device=queries.device)
@@ -82,6 +88,7 @@ class NeighborGrid:
         return counts[:Nq], mx
 
     def fill(self, queries, q_batches, cols, pad_value):
+        queries, q_batches = self._queries("fill", queries, q_batches)
         Nq = int(queries.shape[0])
         out = torch.empty((Nq, int(cols)), dtype=torch.int32, device=queries.device)
         if Nq * int(cols) > 0:
