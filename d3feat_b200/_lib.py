@@ -143,6 +143,21 @@ def row_count_arg(t, name, device):
     return t
 
 
+def publish_ready(device):
+    """Whether a lazily computed cache entry (packed weight image, folded batch norm) that the current stream has just
+    been given to produce may be published. A later hit uses the entry from any thread and stream with no ordering
+    against its producer, so the producer must have finished: the current stream is synchronised once, on the miss,
+    and a hit never waits. While the current stream is captured into a CUDA graph the entry only exists once the graph
+    has been replayed: False, and the caller uses it for this call without publishing it (the graph then carries the
+    producer; an eager warm-up before the capture keeps it out)."""
+    if device.type != "cuda":
+        return True
+    if torch.cuda.is_current_stream_capturing():
+        return False
+    torch.cuda.current_stream(device).synchronize()
+    return True
+
+
 def workspace(nbytes, device):
     return torch.empty((max(int(nbytes), 256),), dtype=torch.uint8, device=device)
 

@@ -50,6 +50,8 @@ def packed_weight(w2d_view_of):
     L = _lib.lib()
     packed = torch.empty((L.d3f_packed_weight_floats(K, N),), dtype=torch.float32, device=w.device)
     _lib.check(L.d3f_pack_weight(_lib.ptr(w), K, N, _lib.ptr(packed), _lib.stream()), "d3f_pack_weight")
+    if not _lib.publish_ready(w.device):
+        return packed
     if hit is None or hit[0]() is not w:
         weakref.finalize(w, _packed_cache.pop, id(w), None)
     _packed_cache[id(w)] = (weakref.ref(w), w._version, packed)
@@ -94,7 +96,9 @@ def _aligned16(t):
     return t.data_ptr() % 16 == 0
 
 
-_pair_cache = {}       # (id(w1), id(w2)) -> (refs, versions, packed image of the folded [w1*s1 ; w2*s2], shift1 + shift2)
+# (id(w1), id(w2)) -> (refs and versions of w1, w2, s1, s2, t1, t2, packed image of the folded [w1*s1 ; w2*s2],
+# shift1 + shift2)
+_pair_cache = {}
 
 
 def unary_pair_convolution(x1, w1, affine1, x2, w2, affine2, alpha, *, rows=None):
@@ -122,18 +126,22 @@ def unary_pair_convolution(x1, w1, affine1, x2, w2, affine2, alpha, *, rows=None
         return unary_convolution(x1, w1, epilogue=(s1, t1, alpha), residual=shortcut, rows=rows)
     key = (id(w1), id(w2))
     hit = _pair_cache.get(key)
-    vers = (w1._version, w2._version, s1._version, s2._version, t1._version, t2._version)
-    if hit is None or hit[0][0]() is not w1 or hit[0][1]() is not w2 or hit[1] != vers:
+    args = (w1, w2, s1, s2, t1, t2)
+    vers = tuple(a._version for a in args)
+    # the fold reads all six tensors: a new affine of other values at version 0 must not reuse an old fold
+    if hit is None or any(r() is not a for r, a in zip(hit[0], args)) or hit[1] != vers:
         folded = torch.cat([w1.double() * s1.double()[None, :], w2.double() * s2.double()[None, :]], 0).float()
         shift = (t1.double() + t2.double()).float().contiguous()
         L = _lib.lib()
         packed = torch.empty((L.d3f_packed_weight_floats(C1 + C2, Cout),), dtype=torch.float32, device=w1.device)
         _lib.check(L.d3f_pack_weight(_lib.ptr(folded.contiguous()), C1 + C2, Cout, _lib.ptr(packed), _lib.stream()),
                    "d3f_pack_weight")
-        if hit is None:
-            weakref.finalize(w1, _pair_cache.pop, key, None)
-        hit = ((weakref.ref(w1), weakref.ref(w2)), vers, packed, shift)
-        _pair_cache[key] = hit
+        fresh = hit is None
+        hit = (tuple(weakref.ref(a) for a in args), vers, packed, shift)
+        if _lib.publish_ready(dev):
+            if fresh:
+                weakref.finalize(w1, _pair_cache.pop, key, None)
+            _pair_cache[key] = hit
     out = torch.empty((N, Cout), dtype=torch.float32, device=x1.device)
     _lib.check(_lib.lib().d3f_unary_pair_forward(_lib.ptr(x1), C1, _lib.ptr(x2), C2, _lib.ptr(hit[2]), N, Cout,
                                                  _lib.ptr(hit[3]), -1.0 if alpha is None else float(alpha),

@@ -1118,11 +1118,19 @@ static AuxStream* aux_stream() {
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return nullptr;
   AuxStream& a = all.dev[dev];
   if (a.stream != nullptr) return &a;
-  if (cudaStreamCreateWithFlags(&a.stream, cudaStreamNonBlocking) != cudaSuccess) { a.stream = nullptr; return nullptr; }
-  for (int i = 0; i < 2; ++i) {
-    cudaEventCreateWithFlags(&a.s1_done[i], cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&a.gemm_done[i], cudaEventDisableTiming);
-  }
+  // The first multi-chunk call of a thread may come while that thread captures a CUDA graph (global capture mode,
+  // as torch.cuda.graph uses). Creating the stream and events is not part of the work being captured, so it runs in
+  // relaxed mode, which a capture in progress neither refuses nor is invalidated by.
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  AuxStream n;
+  bool ok = cudaStreamCreateWithFlags(&n.stream, cudaStreamNonBlocking) == cudaSuccess;
+  for (int i = 0; ok && i < 2; ++i)
+    ok = cudaEventCreateWithFlags(&n.s1_done[i], cudaEventDisableTiming) == cudaSuccess &&
+         cudaEventCreateWithFlags(&n.gemm_done[i], cudaEventDisableTiming) == cudaSuccess;
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  if (!ok) return nullptr;      // the call then runs its chunks on the caller's stream alone
+  a = n;
   return &a;
 }
 

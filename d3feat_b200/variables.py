@@ -3,12 +3,22 @@
 test time, a Saver restores them by name (utils/tester.py:143-162). Here the restored checkpoint is a dict
 {scoped name: array}; the mirrored blocks look their parameters up under the same names."""
 import contextlib
+import threading
 
 import numpy as np
 import torch
 
-_scope = []
-_store = None
+from . import _lib
+
+# The active store and scope are per host thread: two threads running two models must not see each other's scopes
+# (every library call releases the GIL, so their `use_params` / `variable_scope` blocks interleave).
+class _ThreadState(threading.local):
+    def __init__(self):
+        self.scope = []
+        self.store = None
+
+
+_state = _ThreadState()
 
 
 class ParamStore:
@@ -37,41 +47,48 @@ class ParamStore:
 
     def bn_affine(self, scope, eps=1e-6):
         """Inference batch norm folded to y = x*scale + shift (models/network_blocks.py:149-160 with moving
-        statistics): scale = gamma / sqrt(var + eps), shift = beta - mean * scale. Folded in float64."""
-        if scope not in self._bn:
-            pre = scope + "/batch_normalization/"
-            g, b, m, v = (self.t[pre + k].double() for k in ("gamma", "beta", "moving_mean", "moving_variance"))
-            scale = g / torch.sqrt(v + eps)
-            shift = b - m * scale
-            self._bn[scope] = (scale.float().contiguous(), shift.float().contiguous())
-        return self._bn[scope]
+        statistics): scale = gamma / sqrt(var + eps), shift = beta - mean * scale. Folded in float64, once per
+        scope, and again when one of the four tensors is replaced or updated in place."""
+        pre = scope + "/batch_normalization/"
+        src = tuple(self.t[pre + k] for k in ("gamma", "beta", "moving_mean", "moving_variance"))
+        key = (scope, eps)
+        hit = self._bn.get(key)
+        if hit is not None and all(a is b and a._version == v for a, b, v in zip(src, hit[0], hit[1])):
+            return hit[2]
+        g, b, m, v = (a.double() for a in src)
+        scale = g / torch.sqrt(v + eps)
+        shift = b - m * scale
+        res = (scale.float().contiguous(), shift.float().contiguous())
+        if _lib.publish_ready(self.device):
+            self._bn[key] = (src, tuple(a._version for a in src), res)
+        return res
 
 
 @contextlib.contextmanager
 def use_params(store):
-    global _store
-    prev, _store = _store, store
+    prev, _state.store = _state.store, store
     try:
         yield store
     finally:
-        _store = prev
+        _state.store = prev
 
 
 @contextlib.contextmanager
 def variable_scope(name):
-    _scope.append(name)
+    scope = _state.scope
+    scope.append(name)
     try:
         yield
     finally:
-        _scope.pop()
+        scope.pop()
 
 
 def current_scope():
-    return "/".join(_scope)
+    return "/".join(_state.scope)
 
 
 def current_store():
-    return _store
+    return _state.store
 
 
 def scoped(name):
