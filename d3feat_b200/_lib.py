@@ -23,6 +23,8 @@ SYMBOLS = [
     ("d3f_bbox", _I, [_P, _I, _P, _P]),
     ("d3f_grid_subsample_workspace_bytes", _Z, [_I, _I]),
     ("d3f_grid_subsample", _I, [_P, _P, _I, _I, _F, _P, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _Z, _P]),
+    ("d3f_voxel_down_sample_workspace_bytes", _Z, [_I, _I]),
+    ("d3f_voxel_down_sample", _I, [_P, _P, _I, _I, _P, _D, _P, _P, _P, _P, _I, _P, _P, _Z, _P]),
     ("d3f_radius_neighbors_workspace_bytes", _Z, [_I, _I, _F, _P]),
     ("d3f_radius_neighbors_build", _I, [_P, _P, _I, _I, _F, _P, _P, _Z, _P]),
     ("d3f_radius_neighbors_count", _I, [_P, _P, _I, _P, _P, _I, _I, _F, _P, _P, _P, _P, _P]),

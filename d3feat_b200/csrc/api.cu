@@ -55,6 +55,15 @@ int d3f_grid_subsample(const float* pts, const int* batch_len, int B, int N, flo
                         out_classes, out_batch_len, out_M, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
+size_t d3f_voxel_down_sample_workspace_bytes(int N, int B) { return voxel_down_sample_workspace_bytes(N, B); }
+
+int d3f_voxel_down_sample(const float* pts, const int* lengths, int B, int N, const int* n_dev, double voxel_size,
+                          const float* host_bbox, float* out_pts, int* out_lengths, int* out_M, int out_capacity,
+                          int* d_status, void* workspace, size_t workspace_bytes, d3f_stream_t stream) {
+  return voxel_down_sample(pts, lengths, B, N, n_dev, voxel_size, host_bbox, out_pts, out_lengths, out_M, out_capacity,
+                           d_status, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
 size_t d3f_radius_neighbors_workspace_bytes(int Ns, int B, float radius, const float* host_bbox) {
   return radius_neighbors_workspace_bytes(Ns, B, radius, host_bbox);
 }

@@ -38,6 +38,12 @@ int grid_subsample(const float* pts, const int* batch_len, int B, int N, float d
                    cudaStream_t stream, const int* n_dev = nullptr, int out_capacity = -1, int* status = nullptr,
                    const int* start_pre = nullptr);
 
+// ---- voxel.cu ---------------------------------------------------------------------------------------
+size_t voxel_down_sample_workspace_bytes(int N, int B);
+int voxel_down_sample(const float* pts, const int* lengths, int B, int N, const int* n_dev, double voxel_size,
+                      const float* host_bbox, float* out_pts, int* out_lengths, int* out_M, int out_capacity,
+                      int* d_status, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+
 // ---- neighbors.cu -----------------------------------------------------------------------------------
 size_t radius_neighbors_workspace_bytes(int Ns, int B, float radius, const float* host_bbox);
 // ns_dev / nq_dev / pad_dev (optional): actual row counts / the shadow index in device memory; Ns / Nq are then capacities

@@ -20,6 +20,7 @@ from .matching import host_pairs, match_keypoints
 from .registration import ICP_OPTIONS, OPTIONS as REGISTER_OPTIONS, check_icp_options, check_options, icp_pairs, \
     register_pairs
 from .variables import ParamStore, use_params
+from .voxel import VoxelStage, voxel_down_sample
 
 # GraphPipeline(..., keypoints=k) result: descriptors [cap0,32], scores [cap0,1], keypoints (KeypointSet, k per cloud)
 Detections = namedtuple("Detections", "descriptors scores keypoints")
@@ -246,18 +247,27 @@ class GraphPipeline:
     against it, and `res` is an EvaluatedDetections(descriptors, scores, keypoints, matches, registration, refinement,
     evaluation) with that step's per-pair metrics and totals. step() adds the step's totals into a running fp64 vector
     on the caller's stream, in step order; evaluation_totals() reads it (one device->host read, for
-    evaluation.summary(totals, pipe.evaluate_levels, pipe.evaluate_pose_sets)) and reset_evaluation() zeroes it."""
+    evaluation.summary(totals, pipe.evaluate_levels, pipe.evaluate_pose_sets)) and reset_evaluation() zeroes it.
+
+    voxel_size=v (with raw_capacity, the raw rows a slot holds): batches are raw scans. prime / step take the raw
+    points and lengths, and the pyramid graph starts with voxel.voxel_down_sample's static form, which writes the slot's
+    level 0 (points, lengths, row count) on the device: raw scans in, the reference's voxel_down_sample(v) input stage
+    inside the graph, no host step. Capacities and bbox are those of the voxelised level 0 (for_batch sizes them from
+    one voxelised batch); more voxels than capacities[0] set status bit 1, a cloud wider than the bbox allows bit 0.
+    Keypoints, ICP and the evaluation see the voxelised level 0."""
 
     DEPTH = 4
 
     def __init__(self, enc, capacities, n_clouds, bbox, decoder=False, post=None, encoder_streams=2, keypoints=None,
-                 match_pairs=None, register=None, icp=None, evaluate=None):
+                 match_pairs=None, register=None, icp=None, evaluate=None, voxel_size=None, raw_capacity=None):
         if keypoints is not None and not decoder:
             raise ValueError("GraphPipeline: keypoints=%r needs decoder=True (the detection scores)" % (keypoints,))
         if keypoints is not None and int(keypoints) < 1:
             raise ValueError("GraphPipeline: keypoints=%r must be >= 1" % (keypoints,))
         if match_pairs is not None and keypoints is None:
             raise ValueError("GraphPipeline: match_pairs needs keypoints=k (the descriptors it matches)")
+        if voxel_size is not None and raw_capacity is None:
+            raise ValueError("GraphPipeline: voxel_size needs raw_capacity (the raw rows a slot holds)")
         if register is not None:
             if match_pairs is None:
                 raise ValueError("GraphPipeline: register needs match_pairs (the matches it registers)")
@@ -301,6 +311,9 @@ class GraphPipeline:
         self.DEPTH = len(self.s_encs) + 2     # encoders in flight + the pyramid being built + one slot of slack
         self.slots = [pyramid.PyramidBuffers(enc.config, enc.limits, self.caps, self.n_clouds, dev, bbox=self.bbox)
                       for _ in range(self.DEPTH)]
+        # per slot: the raw batch and the voxel stage that writes the slot's level 0
+        self.voxel = (None if voxel_size is None else
+                      [VoxelStage(raw_capacity, self.n_clouds, voxel_size, self.bbox, dev) for _ in range(self.DEPTH)])
         self.g_pyr = [None] * self.DEPTH
         self.g_enc = [None] * self.DEPTH
         self.out = [None] * self.DEPTH          # (inputs, F, res) captured per slot
@@ -322,7 +335,17 @@ class GraphPipeline:
     @classmethod
     def for_batch(cls, enc, points, lengths, slack=1.125, margin=0.05, **kw):
         """Bucket from a representative batch: one exact pass gives the level sizes (capacities = sizes x slack) and
-        the scene bounds (its bbox inflated by `margin` of the extent on every side)."""
+        the scene bounds (its bbox inflated by `margin` of the extent on every side). With voxel_size=v the batch is
+        raw: it is voxelised once (voxel.voxel_down_sample) and sizes the bucket as above, and the raw capacity is its
+        row count x slack rounded up to 256."""
+        if kw.get("voxel_size") is not None:
+            dev = enc.device
+            points = (points if torch.is_tensor(points) else
+                      torch.as_tensor(np.ascontiguousarray(points, np.float32))).to(dev)
+            lengths = (lengths if torch.is_tensor(lengths) else
+                       torch.as_tensor(np.ascontiguousarray(lengths, np.int32))).to(dev)
+            kw.setdefault("raw_capacity", max(-(-int(int(points.shape[0]) * slack) // 256) * 256, 256))
+            points, lengths = voxel_down_sample(points, lengths, kw["voxel_size"])
         inputs = enc.build_inputs(points, lengths)
         sizes = [int(p.shape[0]) for p in inputs["points"]]
         pts = inputs["points"][0]
@@ -333,6 +356,9 @@ class GraphPipeline:
 
     # ---- one slot -----------------------------------------------------------------------------------------
     def _run_pyramid(self, k):
+        if self.voxel is not None:
+            buf = self.slots[k]
+            self.voxel[k].run(buf.points0, buf.lengths0, buf.n0, buf.status)
         return self.enc.build_inputs_static(self.slots[k])
 
     def _run_encoder(self, inputs, k):
@@ -399,21 +425,24 @@ class GraphPipeline:
         if self.done[k] is not None:
             self.done[k].synchronize()        # bounds the host's run-ahead to DEPTH steps (normally long complete)
         buf = self.slots[k]
-        n0 = int(points.shape[0])
-        if n0 > buf.caps[0] or int(lengths.shape[0]) != self.n_clouds:
+        # the batch goes into the slot's level 0, or with voxel_size into its raw buffers
+        dst = (buf.points0, buf.lengths0, buf.n0) if self.voxel is None else \
+            (self.voxel[k].points, self.voxel[k].lengths, self.voxel[k].n)
+        n0, cap = int(points.shape[0]), int(dst[0].shape[0])
+        if n0 > cap or int(lengths.shape[0]) != self.n_clouds:
             raise ValueError("GraphPipeline: batch (%d points, %d clouds) does not fit the bucket (%d, %d)" % (
-                n0, int(lengths.shape[0]), buf.caps[0], self.n_clouds))
+                n0, int(lengths.shape[0]), cap, self.n_clouds))
         if self.g_pyr[k] is None:             # first use of the slot: fill it, then capture its two graphs
-            buf.points0[:n0].copy_(torch.as_tensor(points), non_blocking=True)
-            buf.lengths0.copy_(torch.as_tensor(lengths), non_blocking=True)
-            buf.n0.fill_(n0)
+            dst[0][:n0].copy_(torch.as_tensor(points), non_blocking=True)
+            dst[1].copy_(torch.as_tensor(lengths), non_blocking=True)
+            dst[2].fill_(n0)
             torch.cuda.synchronize(self.enc.device)
             self._capture(k)
         self.s_pyr.wait_event(inputs_ready)
         with torch.cuda.stream(self.s_pyr):
-            buf.points0[:n0].copy_(torch.as_tensor(points), non_blocking=True)
-            buf.lengths0.copy_(torch.as_tensor(lengths), non_blocking=True)
-            buf.n0.fill_(n0)
+            dst[0][:n0].copy_(torch.as_tensor(points), non_blocking=True)
+            dst[1].copy_(torch.as_tensor(lengths), non_blocking=True)
+            dst[2].fill_(n0)
             if truth is not None:
                 self._load_truth(k, truth)
             self.g_pyr[k].replay()

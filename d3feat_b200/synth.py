@@ -7,6 +7,8 @@ There is no network here for 3DMatch / KITTI, so the benchmark shapes are synthe
   (datasets/ThreeDMatch.py:349 open3d voxel_down_sample, out of scope) and cut to exactly ``n_points``.
 * ``lidar_scan(seed, n_points)``     -- KITTI-shaped spinning-lidar scan (ground plane + boxes).
 * ``surface_cloud(seed, n_points)``  -- uniform-on-surfaces cloud for the 1 M-point microbench.
+* ``raw_room_scan(seed, n_raw)`` / ``raw_lidar_scan(seed, n_az)`` -- the same rooms and scans before voxelisation, the
+  inputs of ``voxel.voxel_down_sample`` (0.03 m / 0.3 m).
 
 ``Config`` carries the attributes the reference blocks read from ``utils/config.py`` (values from
 results/Log_contraloss/parameters.txt). ``make_params`` draws weights with the recipe of
@@ -124,34 +126,40 @@ def room_fragment(seed, n_points=30000, dl=0.03):
     return np.ascontiguousarray(vox[rng.permutation(n_points)], np.float32)
 
 
+def _lidar_returns(rng, n_az):
+    """Returns of a 64-beam spinning lidar with n_az azimuth steps over a ground plane and 60 random boxes."""
+    az = np.linspace(0, 2 * np.pi, n_az, endpoint=False)
+    el = np.deg2rad(np.linspace(-24.8, 2.0, 64))
+    A, E = np.meshgrid(az, el)
+    dirs = np.stack([np.cos(E) * np.cos(A), np.cos(E) * np.sin(A), np.sin(E)], -1).reshape(-1, 3)
+    h = 1.73
+    t = np.full(dirs.shape[0], 120.0)
+    down = dirs[:, 2] < -1e-3
+    t[down] = np.minimum(t[down], h / -dirs[down, 2])
+    # axis-aligned boxes (buildings / cars)
+    nb = 60
+    c = np.concatenate([rng.uniform(-70, 70, (nb, 2)), np.zeros((nb, 1))], 1)
+    sz = np.concatenate([rng.uniform(1.5, 12, (nb, 2)), rng.uniform(1.4, 9, (nb, 1))], 1)
+    lo = c - np.array([0.5, 0.5, 0]) * sz - np.array([0, 0, h])
+    hi = lo + sz
+    for b in range(nb):
+        with np.errstate(divide="ignore", invalid="ignore"):
+            t1 = lo[b] / dirs
+            t2 = hi[b] / dirs
+        tn = np.nanmax(np.minimum(t1, t2), 1)
+        tf = np.nanmin(np.maximum(t1, t2), 1)
+        hit = (tn < tf) & (tn > 2.0)
+        t = np.where(hit & (tn < t), tn, t)
+    keep = t < 119.0
+    pts = dirs[keep] * (t[keep, None] + rng.normal(scale=0.02, size=(keep.sum(), 1)))
+    return pts
+
+
 def lidar_scan(seed, n_points=120000, dl=0.30):
     """KITTI-shaped scan: ground plane + boxes seen by a 64-beam spinning lidar, voxelised at dl."""
     rng = np.random.default_rng(5000 + seed)
     for n_az in (2600, 3600, 5200, 8000, 12000, 20000, 32000):
-        az = np.linspace(0, 2 * np.pi, n_az, endpoint=False)
-        el = np.deg2rad(np.linspace(-24.8, 2.0, 64))
-        A, E = np.meshgrid(az, el)
-        dirs = np.stack([np.cos(E) * np.cos(A), np.cos(E) * np.sin(A), np.sin(E)], -1).reshape(-1, 3)
-        h = 1.73
-        t = np.full(dirs.shape[0], 120.0)
-        down = dirs[:, 2] < -1e-3
-        t[down] = np.minimum(t[down], h / -dirs[down, 2])
-        # axis-aligned boxes (buildings / cars)
-        nb = 60
-        c = np.concatenate([rng.uniform(-70, 70, (nb, 2)), np.zeros((nb, 1))], 1)
-        sz = np.concatenate([rng.uniform(1.5, 12, (nb, 2)), rng.uniform(1.4, 9, (nb, 1))], 1)
-        lo = c - np.array([0.5, 0.5, 0]) * sz - np.array([0, 0, h])
-        hi = lo + sz
-        for b in range(nb):
-            with np.errstate(divide="ignore", invalid="ignore"):
-                t1 = lo[b] / dirs
-                t2 = hi[b] / dirs
-            tn = np.nanmax(np.minimum(t1, t2), 1)
-            tf = np.nanmin(np.maximum(t1, t2), 1)
-            hit = (tn < tf) & (tn > 2.0)
-            t = np.where(hit & (tn < t), tn, t)
-        keep = t < 119.0
-        pts = dirs[keep] * (t[keep, None] + rng.normal(scale=0.02, size=(keep.sum(), 1)))
+        pts = _lidar_returns(rng, n_az)
         vox = _voxel_barycenters(pts, dl)
         if vox.shape[0] >= n_points:
             break
@@ -161,6 +169,20 @@ def lidar_scan(seed, n_points=120000, dl=0.30):
     order = np.argsort(rr, kind="stable")
     vox = vox[np.sort(order[:n_points])]
     return np.ascontiguousarray(vox[rng.permutation(n_points)], np.float32)
+
+
+def raw_room_scan(seed, n_raw=300000, box=3.0):
+    """Raw (not voxelised) 3DMatch-shaped fragment: planar patches with 5 mm noise in a `box` m room, about n_raw
+    points in random order (float32 [n,3]). The input of voxel.voxel_down_sample at 0.03 m."""
+    rng = np.random.default_rng(11000 + seed)
+    pts = _sample_patches(rng, 14, box, n_raw)
+    return np.ascontiguousarray(pts[rng.permutation(pts.shape[0])], np.float32)
+
+
+def raw_lidar_scan(seed, n_az=2000):
+    """Raw (not voxelised) KITTI-shaped 64-beam scan with n_az azimuth steps, about 64 * n_az * 0.9 returns in beam
+    order (float32 [n,3]). The input of voxel.voxel_down_sample at 0.3 m."""
+    return np.ascontiguousarray(_lidar_returns(np.random.default_rng(13000 + seed), n_az), np.float32)
 
 
 def surface_cloud(seed, n_points=1000000, box=12.0):

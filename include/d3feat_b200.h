@@ -15,6 +15,9 @@
  *   d3f_grid_subsample        tf_custom_ops/tf_subsampling/tf_batch_subsampling.cpp:8-20,30-122
  *                             tf_custom_ops/tf_subsampling/tf_subsampling.cpp:8-17 (B = 1)
  *                             cpp_wrappers/cpp_subsampling/wrapper.cpp:58-286 (features / classes)
+ *   d3f_voxel_down_sample     open3d.voxel_down_sample of the raw scans: datasets/ThreeDMatch.py:349 (0.03 m),
+ *                             datasets/ETH.py:169 (0.0625 m), datasets/KITTI.py:314-315 (first_subsampling_dl),
+ *                             demo_registration.py:24 (0.03 m)
  *   d3f_radius_neighbors_*    tf_custom_ops/tf_neighbors/tf_batch_neighbors.cpp:8-30,40-116
  *                             tf_custom_ops/tf_neighbors/tf_neighbors.cpp:8-18 (B = 1, pad = -1)
  *   d3f_kpconv_forward        kernels/convolution_ops.py:161-255 (KPConv_ops) + BN/LeakyReLU epilogue
@@ -96,6 +99,38 @@ int d3f_grid_subsample(const float* pts, const int* batch_len, int B, int N, flo
                        const float* host_bbox, float* out_pts, float* out_feats, int* out_classes,
                        int* out_batch_len, int* out_M, void* workspace, size_t workspace_bytes,
                        d3f_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Voxel down-sampling of raw scans, stacked clouds: Open3D 0.7's voxel_down_sample (Geometry/DownSample.cpp), the
+ * input stage of every reference entry point. Per cloud b, from its fp32 rows widened exactly to fp64, each step one
+ * IEEE fp64 operation (true division, no fused multiply-add):
+ *     min_b = per-axis minimum of the cloud's finite rows - voxel_size * 0.5
+ *     i_a   = (int)floor((p_a - min_b,a) / voxel_size)                    (>= 0)
+ *     voxel point = (sum of its rows in fp64, sequentially in input order) / (double)count, rounded to nearest fp32.
+ *   voxel_size is a DOUBLE: voxel_down_sample(x, 0.03) uses the double 0.03; float(0.03) voxelises differently.
+ *   Deviations from Open3D: voxels are emitted per cloud in ascending (iz, iy, ix), not in hash-map order; the output
+ *   is fp32; a row with a non-finite coordinate is dropped (in no voxel, not in the bounds); a voxel_size that is not
+ *   finite and > 0 is D3F_ERR_INVALID (Open3D returns an empty cloud).
+ *   pts[N,3], lengths[B] (device int32), B in [1, 1024]; clouds as in d3f_grid_subsample (rows at or past start[B]
+ *   belong to no cloud, lengths summing past the row count cut the last cloud). n_dev (device, optional): the raw row
+ *   count, N then being the capacity of pts and of every launch.
+ *   host_bbox: host float[6] bounding the clouds. It sizes the sort key: each axis gets the index width of the host
+ *   extent / voxel_size plus a margin, at most 30 bits (so every index fits an int and Open3D's voxel_size * INT_MAX <
+ *   extent guard cannot trigger), and cloud + three axes at most 62 bits; otherwise D3F_ERR_CAPACITY. A cloud merely
+ *   displaced outside host_bbox is still voxelised exactly; one whose own extent needs wider indices overflows.
+ *   Outputs: out_pts[out_capacity,3] (out_capacity < 0: N), out_lengths[B], out_M[1] (device int32).
+ *   Exact form (d_status == NULL): *out_M = the number of voxels, -1 for a key overflow, -2 for more voxels than
+ *   out_capacity; the caller reads it back (the output size is data dependent).
+ *   Static form (d_status != NULL): nothing is read back. *out_M = min(voxels, out_capacity); no row at or past
+ *   out_capacity is written; out_lengths count the written voxels; bit 0 of *d_status is OR-ed for a key overflow,
+ *   bit 1 for more voxels than out_capacity. The launch sequence depends only on (B, N, out_capacity, host_bbox,
+ *   voxel_size): it can be captured in a CUDA graph.
+ *   Argument errors (D3F_ERR_INVALID / _CAPACITY / _WORKSPACE) are returned before any CUDA call.
+ * ------------------------------------------------------------------------------------------- */
+size_t d3f_voxel_down_sample_workspace_bytes(int N, int B);
+int d3f_voxel_down_sample(const float* pts, const int* lengths, int B, int N, const int* n_dev, double voxel_size,
+                          const float* host_bbox, float* out_pts, int* out_lengths, int* out_M, int out_capacity,
+                          int* d_status, void* workspace, size_t workspace_bytes, d3f_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Radius neighbours, stacked clouds (hash grid over the supports, 27-cell scan per query).
