@@ -412,7 +412,9 @@ class GraphPipeline:
         self.kernels_per_step = _lib.launch_count() - n0
         self.g_pyr[k], self.g_enc[k], self.out[k] = gp, ge, (inputs, F, res)
 
-    def _load(self, points, lengths, inputs_ready, truth=None):
+    def _check_batch(self, points, lengths, truth):
+        """ValueError unless the batch fits the slots (raw or level-0 rows, number of clouds) and comes with the truth
+        the pipeline needs. Changes nothing: a rejected batch leaves the pipeline as it was."""
         if self.evaluate is not None and truth is None:
             raise ValueError("GraphPipeline: evaluate needs the truth of every batch (prime(..., truth=...), "
                              "step(..., next_truth=...))")
@@ -420,6 +422,14 @@ class GraphPipeline:
             raise ValueError("GraphPipeline: truth given to a pipeline built without evaluate")
         if truth is not None:
             check_truth(truth, int(self.match_pairs.shape[0]), "GraphPipeline")
+        n0 = int(points.shape[0])
+        cap = int(self.slots[0].points0.shape[0]) if self.voxel is None else self.voxel[0].capacity
+        if n0 > cap or int(lengths.shape[0]) != self.n_clouds:
+            raise ValueError("GraphPipeline: batch (%d points, %d clouds) does not fit the bucket (%d, %d)" % (
+                n0, int(lengths.shape[0]), cap, self.n_clouds))
+
+    def _load(self, points, lengths, inputs_ready, truth=None):
+        """Copy a batch that passed _check_batch into the next slot and replay its pyramid graph."""
         k = self.n_loaded % self.DEPTH
         self.n_loaded += 1
         if self.done[k] is not None:
@@ -428,10 +438,7 @@ class GraphPipeline:
         # the batch goes into the slot's level 0, or with voxel_size into its raw buffers
         dst = (buf.points0, buf.lengths0, buf.n0) if self.voxel is None else \
             (self.voxel[k].points, self.voxel[k].lengths, self.voxel[k].n)
-        n0, cap = int(points.shape[0]), int(dst[0].shape[0])
-        if n0 > cap or int(lengths.shape[0]) != self.n_clouds:
-            raise ValueError("GraphPipeline: batch (%d points, %d clouds) does not fit the bucket (%d, %d)" % (
-                n0, int(lengths.shape[0]), cap, self.n_clouds))
+        n0 = int(points.shape[0])
         if self.g_pyr[k] is None:             # first use of the slot: fill it, then capture its two graphs
             dst[0][:n0].copy_(torch.as_tensor(points), non_blocking=True)
             dst[1].copy_(torch.as_tensor(lengths), non_blocking=True)
@@ -469,11 +476,24 @@ class GraphPipeline:
         return ev
 
     def prime(self, points, lengths, truth=None):
+        self._check_batch(points, lengths, truth)
         self.pending = self._load(points, lengths, self._mark_inputs(), truth)
 
     def step(self, next_points=None, next_lengths=None, pre=None, next_truth=None):
         """Replay encoder(current batch), then load + replay the pyramid of the next batch on the other stream.
-        Returns (result buffer, device level counts) of the current batch, ordered on the caller's stream."""
+        Returns (result buffer, device level counts) of the current batch, ordered on the caller's stream.
+
+        A next batch that does not fit (too many rows, another number of clouds, missing or malformed truth) raises
+        ValueError before anything runs: the current batch stays pending, and the next step() returns it once.
+
+        A batch that outgrows the bucket on the device is not refused: its step runs on a defined truncation and sets
+        the slot's status word (see check()). counts[0] is then at most capacities[0] (with voxel_size, the first
+        capacities[0] voxels in (cloud, iz, iy, ix) order are kept). When subsampling level l - 1 fails, counts[l] is
+        -1 (a cloud wider than the bbox allows, status bit 0) or -2 (more cells than capacities[l], status bit 1), and
+        every deeper count is <= 0: those levels have no rows, their pool and upsample rows name no support, and every
+        output of the step stays finite."""
+        if next_points is not None:
+            self._check_batch(next_points, next_lengths, next_truth)
         k = self.pending
         cur = torch.cuda.current_stream(self.enc.device)
         inputs_ready = self._mark_inputs() if next_points is not None else None
@@ -502,10 +522,18 @@ class GraphPipeline:
 
     def evaluation_totals(self):
         """The running totals of every step since construction or reset_evaluation(), as float64 numpy (one
-        device->host read on the caller's stream): see evaluation.summary."""
-        return self.eval_running.cpu().numpy()
+        device->host read on the caller's stream, after the pyramid of the pending batch): see evaluation.summary.
+        Raises RuntimeError, as check() does, once any batch loaded so far has overflowed the bucket: its totals
+        were computed on truncated clouds."""
+        cur = torch.cuda.current_stream(self.enc.device)
+        cur.wait_stream(self.s_pyr)
+        status = torch.cat([buf.status for buf in self.slots]).to(torch.float64)
+        got = torch.cat([self.eval_running, status]).cpu().numpy()
+        self._raise_on_status(got[self.eval_running.shape[0]:].astype(np.int64))
+        return got[:self.eval_running.shape[0]]
 
     def reset_evaluation(self):
+        """Zero the running totals. The status words stay set: see check()."""
         self.eval_running.zero_()
 
     def drain(self):
@@ -514,10 +542,15 @@ class GraphPipeline:
             s.synchronize()
 
     def check(self):
-        """Raise if any replayed batch overflowed the bucket (synchronises)."""
+        """Raise if any batch loaded so far overflowed the bucket (synchronises). The status words are sticky: they
+        are never cleared, so once one is set check() and evaluation_totals() raise for the rest of the pipeline's
+        life; a bucket that has overflowed has to be rebuilt larger."""
         self.drain()
-        for k, buf in enumerate(self.slots):
-            st = int(buf.status.item())
+        self._raise_on_status([int(buf.status.item()) for buf in self.slots])
+
+    @staticmethod
+    def _raise_on_status(status):
+        for k, st in enumerate(status):
             if st:
                 raise RuntimeError("GraphPipeline: slot %d status %d (%s)" % (
                     k, st, "a cloud wider than the scene bounds" if st & 1 else "a level exceeded its capacity"))
