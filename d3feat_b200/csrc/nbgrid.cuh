@@ -35,6 +35,25 @@ static NbGrid make_grid(const float* host_bbox, float radius) {
 
 constexpr long long kMaxGridCells = 1ll << 27;  // 128 Mi cells total (2 x 4 B tables = 1 GiB)
 
+// Why the 27 cells around a query's cell hold every support with fp32 d2 < r2 (the radius search of neighbors.cu),
+// and up to which axis length. Queries and supports are fp32 points, r2 = fl(r * r), cell edge c = fl(r * 1.001f),
+// inv = fl(1 / c), and along one axis the cell of v is
+//   idx(v) = clamp(floor(Y(v)), 0, n - 1),   Y(v) = fl(fl(v - mn) * inv),
+// monotone in v. A hit has fl(dx * dx) <= d2 < r2 (fp32 sums of non-negative terms), so |fl(q - s)| < r (1 + 2^-24)
+// and |q - s| < r (1 + 2^-23) on every axis. With E(v) = (v - mn) / c exact, (b - a) * inv (1 + 2^-24)^2 <
+// (1 + 3.5 2^-24) / 1.001f < 0.9990012 cells for a hit's coordinates a < b. Each of Y's two roundings has relative
+// error at most u = 2^-24, so Y(b) - Y(a) < 0.9990012 + 4 u E(a): below one cell, and the floors at most one apart,
+// while E(a) < 9.988e-4 / (4 u) = 4189 cells. That covers every pair when n <= 4189 cells per axis: if E(a) >= n,
+// Y(a) >= n (1 - 2u) > n - 1, so a and every b >= a clamp to the edge cell n - 1; if a < mn, E(b) < 1 and Y(b) < 1,
+// so both clamp to cell 0 or b is in cell 0. kMaxScanAxisCells = 4096 keeps a margin; past it a pair inside the
+// radius can sit two cells apart. Distance from the origin does not enter: v and mn are fp32, so only the extent in
+// cells does. Grids past the bound are refused on the host (neighbors.cu).
+constexpr int kMaxScanAxisCells = 4096;
+
+static inline bool radius_scan_complete(const NbGrid& g) {
+  return g.nx <= kMaxScanAxisCells && g.ny <= kMaxScanAxisCells && g.nz <= kMaxScanAxisCells;
+}
+
 __device__ __forceinline__ int cell_coord(float v, float mn, float inv, int n) {
   int c = (int)floorf((v - mn) * inv);
   return min(max(c, 0), n - 1);

@@ -5,6 +5,10 @@
 // 432-440, 1280-1289): every support of the same cloud with d2 < r2, d2 = ((dx*dx)+dy*dy)+dz*dz evaluated in
 // fp32 with separately rounded mul/add (__fmul_rn/__fadd_rn: nvcc would otherwise contract to FMA),
 // r2 = radius*radius in fp32, rows ascending in (d2, index), padded with pad_value.
+//
+// The 27-cell scan is provably complete only while every grid axis has at most kMaxScanAxisCells = 4096 cells (the
+// derivation is beside make_grid, nbgrid.cuh): about 307 m at the 3DMatch level-0 radius 0.075, 3 km at KITTI's 0.75.
+// Longer grids are refused on the host with D3F_ERR_INVALID before any launch, like the fp64 lookup of icp.cu.
 #include <stdlib.h>
 
 #include "nbgrid.cuh"
@@ -78,7 +82,7 @@ size_t radius_neighbors_workspace_bytes(int Ns, int B, float radius, const float
   if (host_bbox == nullptr || !(radius > 0.f) || B < 1) return 0;
   NbGrid g = make_grid(host_bbox, radius);
   long long total = g.ncells * B;
-  if (total > kMaxGridCells) return 0;
+  if (total > kMaxGridCells || !radius_scan_complete(g)) return 0;
   Carver cv(nullptr, ~(size_t)0);
   NbWs w;
   return carve_nb(cv, Ns, B, total, w) + 256;
@@ -95,6 +99,9 @@ int radius_neighbors_build(const float* supports, const int* s_batch_len, int B,
   D3F_REQUIRE(total <= kMaxGridCells, D3F_ERR_CAPACITY,
               "radius_neighbors: grid %d x %d x %d x %d clouds exceeds %lld cells", g.nx, g.ny, g.nz, B,
               kMaxGridCells);
+  D3F_REQUIRE(radius_scan_complete(g), D3F_ERR_INVALID,
+              "radius_neighbors: grid %d x %d x %d has an axis longer than %d cells (of radius * 1.001)", g.nx, g.ny,
+              g.nz, kMaxScanAxisCells);
   D3F_REQUIRE(workspace_bytes >= radius_neighbors_workspace_bytes(Ns, B, radius, host_bbox), D3F_ERR_WORKSPACE,
               "radius_neighbors: workspace too small");
   Carver cv(workspace, workspace_bytes);
@@ -621,6 +628,9 @@ static int query_common(bool fill, const float* queries, const int* q_batch_len,
   NbGrid g = make_grid(host_bbox, radius);
   long long total = g.ncells * B;
   D3F_REQUIRE(total <= kMaxGridCells, D3F_ERR_CAPACITY, "radius_neighbors: grid too large");
+  D3F_REQUIRE(radius_scan_complete(g), D3F_ERR_INVALID,
+              "radius_neighbors: grid %d x %d x %d has an axis longer than %d cells (of radius * 1.001)", g.nx, g.ny,
+              g.nz, kMaxScanAxisCells);
   Carver cv(const_cast<void*>(workspace), ~(size_t)0);
   NbWs w;
   carve_nb(cv, Ns, B, total, w);

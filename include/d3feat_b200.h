@@ -141,7 +141,9 @@ int d3f_voxel_down_sample(const float* pts, const int* lengths, int B, int N, co
  *   Clouds as in d3f_grid_subsample: supports at or past the end of the last support cloud are in no cloud and
  *   never returned; a query at or past the end of the last query cloud gets count 0 and a row of padding; lengths
  *   summing past the row count cut the last cloud there. host_bbox sizes the grid; points outside it are clamped
- *   into its edge cells, which only adds candidates, so results stay exact.
+ *   into its edge cells, which only adds candidates, so results stay exact. A host_bbox with more than 4096
+ *   cells of radius * 1.001 on one axis is refused (D3F_ERR_INVALID; workspace_bytes returns 0): past that length
+ *   fp32 cell indices can put two points within the radius two cells apart (nbgrid.cuh).
  *
  *   Two-phase use for the exact reference shape [Nq, max count]:
  *     d3f_radius_neighbors_build  -> grid over the supports in `workspace`
