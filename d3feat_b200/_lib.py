@@ -40,6 +40,12 @@ SYMBOLS = [
     ("d3f_kpconv_deform_forward", _I, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _I, _I, _P, _P,
                                        _P, _F, _P, _P, _Z, _P, _P, _P]),
     ("d3f_unary_forward", _I, [_P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _F, _P, _P, _P]),
+    ("d3f_kpconv_backward_workspace_bytes", _Z, [_I, _I, _I, _I, _I, _I, _I]),
+    ("d3f_kpconv_reverse_width", _I, [_P, _I, _I, _I, C.POINTER(C.c_int), _P, _Z, _P, _P, _P]),
+    ("d3f_kpconv_backward", _I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _I, _I, _I, _I, _P, _P, _P,
+                                 _Z, _P, _P, _P]),
+    ("d3f_unary_backward_workspace_bytes", _Z, [_I, _I, _I]),
+    ("d3f_unary_backward", _I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _Z, _P, _P]),
     ("d3f_ind_max_pool_workspace_bytes", _Z, [_I]),
     ("d3f_ind_max_pool", _I, [_P, _P, _I, _I, _I, _I, _P, _P, _Z, _P, _P, _P]),
     ("d3f_closest_pool", _I, [_P, _P, _I, _I, _I, _I, _P, _P, _P, _P]),

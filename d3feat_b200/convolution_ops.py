@@ -13,10 +13,16 @@ Extensions (keyword-only, default off, so reference call sites work unchanged):
   epilogue=(bn_scale, bn_shift, leaky_alpha)  -- fuse inference batch-norm + LeakyReLU into the kernel
   residual=tensor                             -- (unary only) fused shortcut add before the LeakyReLU
 
+Gradients: with grad mode on and `features` or `K_values` requiring grad, KPConv_ops / KPConv and unary_convolution
+run through torch.autograd.Functions whose backward is kpconv_backward / unary_backward (sm_90a kernels, bitwise
+deterministic). Otherwise the call is the plain forward, the same kernels. Differentiating through an epilogue, a
+bias, a residual, the deformable ops or unary_pair_convolution raises NotImplementedError.
+
 Tensors: contiguous CUDA float32 / int32. The kernel points of a KPConv are a restored, non-trainable
 variable in the reference (:145-148); here they come from the active ParamStore under
 '<scope>/kernel_points' or, without a store, from the seeded generator in synth.kernel_points.
 """
+import ctypes as C
 import os
 import weakref
 
@@ -77,6 +83,9 @@ def unary_convolution(features, K_values, *, epilogue=None, residual=None, rows=
     """features[N,Cin] @ K_values[Cin,Cout] (tf.matmul, :90-99).
     rows (extension): int32 device scalar holding the actual row count when `features` is a capacity-sized buffer."""
     op = "unary_convolution"
+    if _grad_wanted(features, K_values, residual, *(epilogue or ())):
+        _refuse_grad(op, epilogue=epilogue, residual=residual)
+        return _UnaryFn.apply(features, K_values, rows)
     x = _lib.tensor_arg(features, op + ": features", _F32, (None, None))
     dev = x.device
     N, Cin = x.shape
@@ -90,6 +99,61 @@ def unary_convolution(features, K_values, *, epilogue=None, residual=None, rows=
                                             None, _lib.ptr(res), alpha, _lib.ptr(out), _lib.stream(), _lib.ptr(rows)),
                "d3f_unary_forward")
     return out
+
+
+def _grad_wanted(*tensors):
+    return torch.is_grad_enabled() and any(torch.is_tensor(t) and t.requires_grad for t in tensors)
+
+
+def _refuse_grad(op, **unsupported):
+    """NotImplementedError when a gradient would have to pass through something that has none here."""
+    given = sorted(k for k, v in unsupported.items() if v is not None)
+    if given:
+        raise NotImplementedError("%s: no gradient through %s; call it without them (or under torch.no_grad())" % (
+            op, ", ".join(k + "=" for k in given)))
+
+
+def _refuse_op_grad(op, *tensors):
+    if _grad_wanted(*tensors):
+        raise NotImplementedError("%s has no backward pass; call it under torch.no_grad() or on detached tensors" % op)
+
+
+def unary_backward(features, K_values, grad_out, *, rows=None, features_grad=True, weights_grad=True):
+    """Gradients of unary_convolution(features, K_values, rows=rows) for the output gradient grad_out[N, Cout]:
+    (dL/dfeatures = grad_out @ K_values^T, dL/dK_values = features^T @ grad_out), either None when not asked for.
+    With rows, rows at or past the count of dL/dfeatures are zero and those of features / grad_out are not read."""
+    op = "unary_backward"
+    x = _lib.tensor_arg(features, op + ": features", _F32, (None, None))
+    dev = x.device
+    N, Cin = x.shape
+    w = _lib.tensor_arg(K_values, op + ": K_values", _F32, (Cin, None), dev)
+    Cout = w.shape[1]
+    g = _lib.tensor_arg(grad_out, op + ": grad_out", _F32, (N, Cout), dev)
+    rows = _lib.row_count_arg(rows, op + ": rows", dev)
+    dx = torch.empty((N, Cin), dtype=torch.float32, device=dev) if features_grad else None
+    dw = torch.empty((Cin, Cout), dtype=torch.float32, device=dev) if weights_grad else None
+    if dx is None and dw is None:
+        return None, None
+    L = _lib.lib()
+    ws = _lib.workspace(L.d3f_unary_backward_workspace_bytes(N, Cin, Cout), dev)
+    _lib.check(L.d3f_unary_backward(_lib.ptr(x), _lib.ptr(w), _lib.ptr(g), N, Cin, Cout, int(USE_TENSOR_CORES),
+                                    _lib.ptr(dx), _lib.ptr(dw), _lib.ptr(ws), ws.numel(), _lib.stream(),
+                                    _lib.ptr(rows)), "d3f_unary_backward")
+    return dx, dw
+
+
+class _UnaryFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, features, K_values, rows):
+        ctx.save_for_backward(features, K_values, rows)
+        return unary_convolution(features, K_values, rows=rows)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        features, K_values, rows = ctx.saved_tensors
+        dx, dw = unary_backward(features, K_values, grad_out, rows=rows, features_grad=ctx.needs_input_grad[0],
+                                weights_grad=ctx.needs_input_grad[1])
+        return dx, dw, None
 
 
 def _aligned16(t):
@@ -109,6 +173,7 @@ def unary_pair_convolution(x1, w1, affine1, x2, w2, affine2, alpha, *, rows=None
     tensor-core path, when the channel counts do not tile, or when x1 or x2 does not start on a 16-byte boundary (the
     one-GEMM kernel fetches both by TMA; a lone unary_convolution then runs its CUDA-core GEMM on that operand)."""
     op = "unary_pair_convolution"
+    _refuse_op_grad(op, x1, w1, x2, w2, *affine1, *affine2)
     x1 = _lib.tensor_arg(x1, op + ": x1", _F32, (None, None))
     dev = x1.device
     N, C1 = x1.shape
@@ -183,6 +248,10 @@ def KPConv_ops(query_points, support_points, neighbors_indices, features, K_poin
     capacity-sized buffers (the shadow index is then the actual support count)."""
     _check_enums(KP_influence, aggregation_mode)
     op = "KPConv_ops"
+    if _grad_wanted(features, K_values, bias, *(epilogue or ())):
+        _refuse_grad(op, epilogue=epilogue, bias=bias)
+        return _KPConvFn.apply(query_points, support_points, neighbors_indices, features, K_points, K_values,
+                               KP_extent, KP_influence, aggregation_mode, query_order, rows_q, rows_s)
     q, s, idx, f, Kp, W, query_order, rows_q, rows_s = _kpconv_args(
         op, query_points, support_points, neighbors_indices, features, K_points, K_values, query_order, rows_q, rows_s)
     Nq, Ns, H = q.shape[0], s.shape[0], idx.shape[1]
@@ -201,12 +270,68 @@ def KPConv_ops(query_points, support_points, neighbors_indices, features, K_poin
     return out
 
 
+def kpconv_backward(query_points, support_points, neighbors_indices, features, K_points, K_values, KP_extent,
+                    KP_influence, aggregation_mode, grad_out, *, rows_q=None, rows_s=None, features_grad=True,
+                    weights_grad=True):
+    """Gradients of KPConv_ops(...) (no epilogue, no bias) for the output gradient grad_out[Nq, Cout]:
+    (dL/dfeatures [Ns, Cin], dL/dK_values [K, Cin, Cout]), either None when not asked for. The neighbour count nn of
+    the normalisation is held constant; points, kernel points and indices get no gradient. Rows of dL/dfeatures that
+    no query reaches, or at or past rows_s, are zero; rows of grad_out at or past rows_q are not read.
+    The feature gradient runs a KPConv over the transposed neighbourhood, whose width (the largest number of
+    neighbour entries naming one support) is read back to the host once per call: one synchronisation of the current
+    stream. The weight gradient alone does not synchronise."""
+    _check_enums(KP_influence, aggregation_mode)
+    op = "kpconv_backward"
+    q, s, idx, f, Kp, W, _, rows_q, rows_s = _kpconv_args(
+        op, query_points, support_points, neighbors_indices, features, K_points, K_values, None, rows_q, rows_s)
+    Nq, Ns, H = q.shape[0], s.shape[0], idx.shape[1]
+    K, Cin, Cout = W.shape
+    g = _lib.tensor_arg(grad_out, op + ": grad_out", _F32, (Nq, Cout), q.device)
+    df = torch.empty((Ns, Cin), dtype=torch.float32, device=q.device) if features_grad else None
+    dW = torch.empty((K, Cin, Cout), dtype=torch.float32, device=q.device) if weights_grad else None
+    if df is None and dW is None:
+        return None, None
+    L = _lib.lib()
+    Hr = 0
+    if df is not None:
+        ws = _lib.workspace(L.d3f_kpconv_backward_workspace_bytes(Nq, Ns, H, K, Cin, Cout, 0), q.device)
+        width = C.c_int(0)
+        _lib.check(L.d3f_kpconv_reverse_width(_lib.ptr(idx), Nq, Ns, H, C.byref(width), _lib.ptr(ws), ws.numel(),
+                                              _lib.stream(), _lib.ptr(rows_q), _lib.ptr(rows_s)),
+                   "d3f_kpconv_reverse_width")
+        Hr = int(width.value)
+    ws = _lib.workspace(L.d3f_kpconv_backward_workspace_bytes(Nq, Ns, H, K, Cin, Cout, Hr), q.device)
+    _lib.check(L.d3f_kpconv_backward(_lib.ptr(q), _lib.ptr(s), _lib.ptr(idx), _lib.ptr(f), _lib.ptr(Kp), _lib.ptr(W),
+                                     _lib.ptr(g), Nq, Ns, H, Hr, K, Cin, Cout, float(KP_extent),
+                                     _INFLUENCE[KP_influence], _MODE[aggregation_mode], 1, int(USE_TENSOR_CORES),
+                                     _lib.ptr(df), _lib.ptr(dW), _lib.ptr(ws), ws.numel(), _lib.stream(),
+                                     _lib.ptr(rows_q), _lib.ptr(rows_s)), "d3f_kpconv_backward")
+    return df, dW
+
+
+class _KPConvFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, s, idx, f, Kp, W, extent, influence, mode, query_order, rows_q, rows_s):
+        ctx.save_for_backward(q, s, idx, f, Kp, W, rows_q, rows_s)
+        ctx.conf = (extent, influence, mode)
+        return KPConv_ops(q, s, idx, f, Kp, W, extent, influence, mode, query_order=query_order, rows_q=rows_q,
+                          rows_s=rows_s)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        q, s, idx, f, Kp, W, rows_q, rows_s = ctx.saved_tensors
+        df, dW = kpconv_backward(q, s, idx, f, Kp, W, *ctx.conf, grad_out, rows_q=rows_q, rows_s=rows_s,
+                                 features_grad=ctx.needs_input_grad[3], weights_grad=ctx.needs_input_grad[5])
+        return None, None, None, df, None, dW, None, None, None, None, None, None
+
+
 def KPConv_deform_ops(query_points, support_points, neighbors_indices, features, K_points, offsets, modulations,
                       K_values, KP_extent, KP_influence, mode, *, epilogue=None, query_order=None, rows_q=None,
                       rows_s=None):
     """Deformable second stage (:379-499)."""
     _check_enums(KP_influence, mode)
     op = "KPConv_deform_ops"
+    _refuse_op_grad(op, features, K_values, offsets, modulations)
     q, s, idx, f, Kp, W, query_order, rows_q, rows_s = _kpconv_args(
         op, query_points, support_points, neighbors_indices, features, K_points, K_values, query_order, rows_q, rows_s)
     Nq, Ns, H = q.shape[0], s.shape[0], idx.shape[1]
@@ -258,6 +383,7 @@ def KPConv_deformable(query_points, support_points, neighbors_indices, features,
                       KP_extent=1.0, KP_influence="linear", aggregation_mode="sum", modulated=False, *,
                       epilogue=None, query_order=None, rows_q=None, rows_s=None):
     """:258-376 -- rigid KPConv producing 3K (4K if modulated) offsets (+ bias), then the deformed conv."""
+    _refuse_op_grad("KPConv_deformable", features, K_values)
     K_radius = 1.5 * KP_extent
     num_kpoints = int(K_values.shape[0])
     points_dim = int(query_points.shape[1])

@@ -202,6 +202,40 @@ int d3f_unary_pair_forward(const float* x1, int Cin1, const float* x2, int Cin2,
   return tc_gemm(x1, W_packed, out, N, Cout, Cin1 + Cin2, ep, (cudaStream_t)stream, nullptr, x2, Cin1);
 }
 
+size_t d3f_kpconv_backward_workspace_bytes(int Nq, int Ns, int H, int K, int Cin, int Cout, int Hr) {
+  return kpconv_backward_workspace_bytes(Nq, Ns, H, K, Cin, Cout, Hr);
+}
+
+int d3f_kpconv_reverse_width(const int* idx, int Nq, int Ns, int H, int* width, void* workspace,
+                             size_t workspace_bytes, d3f_stream_t stream, const int* nq_dev, const int* ns_dev) {
+  return kpconv_reverse_width(idx, Nq, Ns, H, width, workspace, workspace_bytes, (cudaStream_t)stream, nq_dev, ns_dev);
+}
+
+int d3f_kpconv_backward(const float* q, const float* s, const int* idx, const float* feat, const float* Kp,
+                        const float* W, const float* dout, int Nq, int Ns, int H, int Hr, int K, int Cin, int Cout,
+                        float extent, int influence, int mode, int normalize, int tensor_cores, float* dfeat,
+                        float* dW, void* workspace, size_t workspace_bytes, d3f_stream_t stream, const int* nq_dev,
+                        const int* ns_dev) {
+  D3F_REQUIRE(Nq == 0 || Ns == 0 || (dfeat == nullptr && dW == nullptr) ||
+                  (q && s && idx && feat && Kp && W && dout && workspace),
+              D3F_ERR_INVALID, "d3f_kpconv_backward: null pointer");
+  return kpconv_backward(q, s, idx, feat, Kp, W, dout, Nq, Ns, H, Hr, K, Cin, Cout, extent, influence, mode, normalize,
+                         tensor_cores, dfeat, dW, workspace, workspace_bytes, (cudaStream_t)stream, nq_dev, ns_dev);
+}
+
+size_t d3f_unary_backward_workspace_bytes(int N, int Cin, int Cout) {
+  return unary_backward_workspace_bytes(N, Cin, Cout);
+}
+
+int d3f_unary_backward(const float* x, const float* W, const float* dout, int N, int Cin, int Cout, int tensor_cores,
+                       float* dx, float* dW, void* workspace, size_t workspace_bytes, d3f_stream_t stream,
+                       const int* n_dev) {
+  D3F_REQUIRE(N == 0 || (dx == nullptr && dW == nullptr) || (x && W && dout && workspace), D3F_ERR_INVALID,
+              "d3f_unary_backward: null pointer");
+  return unary_backward(x, W, dout, N, Cin, Cout, tensor_cores, dx, dW, workspace, workspace_bytes,
+                        (cudaStream_t)stream, n_dev);
+}
+
 size_t d3f_ind_max_pool_workspace_bytes(int C) { return sizeof(unsigned) * ((size_t)(C > 0 ? C : 1) + 1); }
 
 int d3f_ind_max_pool(const float* x, const int* inds, int N1, int N2, int H, int C, float* out, void* workspace,

@@ -1149,6 +1149,53 @@ static int chunk_queries(int K, int Cin) {
   return (int)(n / 128 * 128);
 }
 
+int kpconv_chunk_queries(int K, int Cin) { return chunk_queries(K, Cin); }
+
+// The support pack of a layer (s4[Ns+1]: x, y, z and the normalisation flag, or the feature itself for the first
+// layer). The backward pass packs with this same function, so its neighbour count uses the forward's predicate.
+int kpconv_prep_supports(bool deform, const float* s, const float* feat, int Ns, const int* ns_dev, int K, int Cin,
+                         int normalize, float4* s4, cudaStream_t stream) {
+  const bool norm = normalize != 0 && !deform;
+  const bool first_layer = Cin == 1 && !deform && K == 15;
+  int pmode = first_layer ? 2 : (norm ? 1 : 0);
+  const float shadow = deform ? 1000.f : 1e6f;
+  const bool vec = pmode == 1 && Cin % 4 == 0 && Cin >= 32 && (reinterpret_cast<uintptr_t>(feat) & 15) == 0;
+  if (vec && Cin < 64)
+    prep_supports_vec_kernel<8><<<ceil_div((Ns + 1) * 8, 256), 256, 0, stream>>>(s, feat, Ns, ns_dev, Cin, shadow, s4);
+  else if (vec && Cin < 128)
+    prep_supports_vec_kernel<16><<<ceil_div((Ns + 1) * 16, 256), 256, 0, stream>>>(s, feat, Ns, ns_dev, Cin, shadow, s4);
+  else if (vec)
+    prep_supports_vec_kernel<32><<<ceil_div((Ns + 1) * 32, 256), 256, 0, stream>>>(s, feat, Ns, ns_dev, Cin, shadow, s4);
+  else
+    prep_supports_kernel<<<ceil_div((Ns + 1) * 32, 256), 256, 0, stream>>>(s, feat, Ns, ns_dev, Cin, pmode, shadow, s4);
+  D3F_LAUNCH_CHECK("prep_supports_kernel");
+  return D3F_OK;
+}
+
+// Stage 1 of a rigid layer on its own: wf[n1 - n0, K*Cin] for the query slots [n0, n1), in the forward's query order
+// (none here: slot = query), no neighbour count. The weight gradient re-derives wf with it.
+int kpconv_stage1_wf(const float* q, const float4* s4, const int* idx, const float* feat, const float* Kp, int Nq, int Ns,
+                     int H, int K, int Cin, float extent, int influence, int mode, int n0, int n1, float* wf,
+                     cudaStream_t stream, const int* nq_dev, const int* ns_dev) {
+  Stage1Params p;
+  p.q = q; p.s4 = s4; p.idx = idx; p.feat = feat; p.count_nn = 0;
+  p.Kp = Kp; p.offsets = nullptr; p.modulations = nullptr;
+  p.Nq = Nq; p.Ns = Ns; p.H = H; p.Cin = Cin;
+  p.n0 = n0; p.n1 = n1;
+  p.order = nullptr;
+  p.extent = extent;
+  p.inv_scale = 1.f / (2.f * extent);
+  float sigma = extent * 0.3f;
+  p.gauss_inv = 1.f / (2.f * sigma * sigma + 1e-9f);
+  p.influence = influence;
+  p.closest = mode == D3F_MODE_CLOSEST;
+  p.shadow = 1e6f;
+  p.wf = wf;
+  p.inv_nn = nullptr;
+  p.nq_dev = nq_dev; p.ns_dev = ns_dev;
+  return launch_stage1<false>(K, p, stream);
+}
+
 size_t kpconv_workspace_bytes(int Nq, int Ns, int H, int K, int Cin, int Cout) {
   (void)H; (void)Cout;
   int chunk = chunk_queries(K, Cin);
@@ -1193,19 +1240,8 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
   float* split_ws = split_floats ? cv.take<float>(split_floats) : nullptr;
   const bool norm = normalize != 0 && !deform;
   {
-    const bool first_layer = Cin == 1 && !deform && K == 15;
-    int pmode = first_layer ? 2 : (norm ? 1 : 0);
-    const float shadow = deform ? 1000.f : 1e6f;
-    const bool vec = pmode == 1 && Cin % 4 == 0 && Cin >= 32 && (reinterpret_cast<uintptr_t>(feat) & 15) == 0;
-    if (vec && Cin < 64)
-      prep_supports_vec_kernel<8><<<ceil_div((Ns + 1) * 8, 256), 256, 0, stream>>>(s, feat, Ns, ns_dev, Cin, shadow, s4);
-    else if (vec && Cin < 128)
-      prep_supports_vec_kernel<16><<<ceil_div((Ns + 1) * 16, 256), 256, 0, stream>>>(s, feat, Ns, ns_dev, Cin, shadow, s4);
-    else if (vec)
-      prep_supports_vec_kernel<32><<<ceil_div((Ns + 1) * 32, 256), 256, 0, stream>>>(s, feat, Ns, ns_dev, Cin, shadow, s4);
-    else
-      prep_supports_kernel<<<ceil_div((Ns + 1) * 32, 256), 256, 0, stream>>>(s, feat, Ns, ns_dev, Cin, pmode, shadow, s4);
-    D3F_LAUNCH_CHECK("prep_supports_kernel");
+    const int rc = kpconv_prep_supports(deform, s, feat, Ns, ns_dev, K, Cin, normalize, s4, stream);
+    if (rc) return rc;
   }
   if (Cin == 1 && !deform && K == 15) {
     Cin1Params c1;

@@ -80,6 +80,27 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
                         float* out, void* workspace, size_t workspace_bytes, cudaStream_t stream,
                         const int* nq_dev = nullptr, const int* ns_dev = nullptr);
 
+// building blocks the backward pass shares with the forward (kpconv.cu)
+int kpconv_chunk_queries(int K, int Cin);
+int kpconv_prep_supports(bool deform, const float* s, const float* feat, int Ns, const int* ns_dev, int K, int Cin,
+                         int normalize, float4* s4, cudaStream_t stream);
+int kpconv_stage1_wf(const float* q, const float4* s4, const int* idx, const float* feat, const float* Kp, int Nq, int Ns,
+                     int H, int K, int Cin, float extent, int influence, int mode, int n0, int n1, float* wf,
+                     cudaStream_t stream, const int* nq_dev = nullptr, const int* ns_dev = nullptr);
+
+// ---- kpconv_grad.cu (feature and weight gradients of rigid KPConv and of the unary convolution) ----------
+size_t kpconv_backward_workspace_bytes(int Nq, int Ns, int H, int K, int Cin, int Cout, int Hr);
+int kpconv_reverse_width(const int* idx, int Nq, int Ns, int H, int* width, void* workspace, size_t workspace_bytes,
+                         cudaStream_t stream, const int* nq_dev, const int* ns_dev);
+int kpconv_backward(const float* q, const float* s, const int* idx, const float* feat, const float* Kp, const float* W,
+                    const float* dout, int Nq, int Ns, int H, int Hr, int K, int Cin, int Cout, float extent,
+                    int influence, int mode, int normalize, int tensor_cores, float* dfeat, float* dW, void* workspace,
+                    size_t workspace_bytes, cudaStream_t stream, const int* nq_dev, const int* ns_dev);
+size_t unary_backward_workspace_bytes(int N, int Cin, int Cout);
+int unary_backward(const float* x, const float* W, const float* dout, int N, int Cin, int Cout, int tensor_cores,
+                   float* dx, float* dW, void* workspace, size_t workspace_bytes, cudaStream_t stream,
+                   const int* n_dev);
+
 // ---- kpconv_fused.cu (one persistent kernel per layer: gather + correlation + wgmma contraction) -------
 bool kpconv_fused_supported(int Nq, int H, int K, int Cin, int Cout, int influence, int mode, const float* feat,
                             const float* W, const float* out, const int* query_order);

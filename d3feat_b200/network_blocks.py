@@ -54,6 +54,7 @@ _F32, _I32 = torch.float32, torch.int32
 
 
 def _pool_args(op, x, inds, rows_x, rows_out):
+    conv_ops._refuse_op_grad(op, x)
     x = _lib.tensor_arg(x, op + ": x", _F32, (None, None))
     inds = _lib.tensor_arg(inds, op + ": inds", _I32, (None, None), x.device)
     return (x, inds, _lib.row_count_arg(rows_x, op + ": rows_x", x.device),

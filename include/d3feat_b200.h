@@ -25,6 +25,8 @@
  *   d3f_kpconv_deform_forward kernels/convolution_ops.py:379-499 (KPConv_deform_ops)
  *   d3f_unary_forward         kernels/convolution_ops.py:90-99 + models/network_blocks.py:207-219,
  *                             :343-368 (conv3 + shortcut add + LeakyReLU)
+ *   d3f_kpconv_backward,      feature and weight gradients of KPConv_ops and unary_convolution (what tf.gradients
+ *   d3f_unary_backward        gives the training scripts, training_3DMatch.py / utils/trainer.py)
  *   d3f_ind_max_pool          models/network_blocks.py:51-66
  *   d3f_closest_pool          models/network_blocks.py:69-83
  *   d3f_l2_normalize          models/D3Feat.py:65
@@ -270,6 +272,38 @@ int d3f_unary_forward(const float* x, const float* W, const float* W_packed, int
                       const float* bn_scale, const float* bn_shift, const float* bias,
                       const float* residual, float leaky_alpha, float* out, d3f_stream_t stream,
                       const int* n_dev);
+
+/* ---------------------------------------------------------------------------------------------
+ * Gradients of rigid KPConv (d3f_kpconv_forward without epilogue or bias) and of the unary convolution.
+ *   G[q,o] = dout[q,o] / nn[q] (nn as the forward counts it; normalize = 0: 1), held constant
+ *   dW[k,c,o] = sum_q wf[q,k,c] G[q,o]          wf[q,k,c] = sum_h w(q,h,k) feat[idx[q,h],c]
+ *   dfeat[s,c] = sum_{(q,h): idx[q,h]=s} sum_k w(q,h,k) sum_o G[q,o] W[k,c,o]
+ * Points, kernel points and indices get no gradient. Shadow entries, rows at or past nq_dev and indices at or past
+ * ns_dev contribute nothing; dfeat rows no query reaches and rows at or past ns_dev are zero; dout rows at or past
+ * nq_dev are never read. dfeat or dW may be NULL (not computed). Bitwise deterministic (no float atomics).
+ * The feature gradient is a forward KPConv over the transposed neighbourhood, whose width Hr (the largest number of
+ * (q, h) entries naming one support) depends on the data:
+ *   d3f_kpconv_reverse_width  computes Hr and copies it to the host int *width: it SYNCHRONISES the stream. Its
+ *                             workspace is d3f_kpconv_backward_workspace_bytes(Nq, Ns, H, K, Cin, Cout, 0) or more.
+ *   d3f_kpconv_backward       takes that Hr (a smaller value drops reverse entries) and a workspace of
+ *                             d3f_kpconv_backward_workspace_bytes(..., Hr). Does not synchronise.
+ * tensor_cores != 0: the transposed contraction runs on the 3xTF32 wgmma GEMM (as a non-NULL W_packed selects in the
+ * forward), 0: the CUDA-core fp32 GEMM. The weight gradient is fp32 FFMA, fresh accumulators every 64 rows, partials
+ * of 2048 rows summed in float64 in a fixed order.
+ * Unary: dx = dout @ W^T (rows at or past n_dev stay zero), dW = x^T @ dout over the rows below n_dev.
+ * ------------------------------------------------------------------------------------------- */
+size_t d3f_kpconv_backward_workspace_bytes(int Nq, int Ns, int H, int K, int Cin, int Cout, int Hr);
+int d3f_kpconv_reverse_width(const int* idx, int Nq, int Ns, int H, int* width, void* workspace,
+                             size_t workspace_bytes, d3f_stream_t stream, const int* nq_dev, const int* ns_dev);
+int d3f_kpconv_backward(const float* q, const float* s, const int* idx, const float* feat, const float* Kp,
+                        const float* W, const float* dout, int Nq, int Ns, int H, int Hr, int K, int Cin, int Cout,
+                        float extent, int influence, int mode, int normalize, int tensor_cores, float* dfeat,
+                        float* dW, void* workspace, size_t workspace_bytes, d3f_stream_t stream, const int* nq_dev,
+                        const int* ns_dev);
+size_t d3f_unary_backward_workspace_bytes(int N, int Cin, int Cout);
+int d3f_unary_backward(const float* x, const float* W, const float* dout, int N, int Cin, int Cout, int tensor_cores,
+                       float* dx, float* dW, void* workspace, size_t workspace_bytes, d3f_stream_t stream,
+                       const int* n_dev);
 
 /* out[N2,C] = max_h x'[inds[n,h]] with x' = x || colmin(x) (shadow index = N1).
  * workspace: C floats. */
