@@ -54,6 +54,16 @@ SYMBOLS = [
     ("d3f_detection_scores_workspace_bytes", _Z, [_I, _I]),
     ("d3f_detection_scores", _I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P, _P]),
     ("d3f_affine_leaky", _I, [_P, _I, _I, _P, _P, _P, _F, _P, _P, _P]),
+    ("d3f_batch_norm_train_workspace_bytes", _Z, [_I, _I]),
+    ("d3f_batch_norm_train_forward", _I, [_P, _I, _I, _P, _P, _P, _P, _F, _F, _P, _F, _P, _P, _P, _P, _Z, _P]),
+    ("d3f_batch_norm_train_backward", _I, [_P, _P, _P, _I, _I, _P, _P, _P, _F, _P, _P, _P, _P, _P, _Z, _P]),
+    ("d3f_ind_max_pool_backward_workspace_bytes", _Z, [_I, _I, _I, _I]),
+    ("d3f_ind_max_pool_backward", _I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P]),
+    ("d3f_gather_rows_backward_workspace_bytes", _Z, [_I, _I]),
+    ("d3f_gather_rows_backward", _I, [_P, _P, _I, _I, _I, _P, _P, _Z, _P]),
+    ("d3f_l2_normalize_backward", _I, [_P, _P, _I, _I, _F, _P, _P]),
+    ("d3f_detection_scores_backward_workspace_bytes", _Z, [_I, _I, _I, _I]),
+    ("d3f_detection_scores_backward", _I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P]),
     ("d3f_select_keypoints_workspace_bytes", _Z, [_I, _I]),
     ("d3f_select_keypoints", _I, [_P, _P, _I, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _Z, _P, _P]),
     ("d3f_match_descriptors_workspace_bytes", _Z, [_I, _I]),

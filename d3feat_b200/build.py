@@ -11,7 +11,7 @@ LIB = os.path.join(_HERE, "libd3feat_b200.so")
 _STAMP = os.path.join(_HERE, "csrc", ".build_stamp")
 
 SOURCES = ["api.cu", "sort.cu", "grid.cu", "neighbors.cu", "kpconv.cu", "kpconv_fused.cu", "gemm.cu", "pool.cu", "tc_gemm.cu", "pyramid.cu",
-           "keypoints.cu", "matching.cu", "registration.cu", "icp.cu", "evaluation.cu", "voxel.cu", "kpconv_grad.cu"]
+           "keypoints.cu", "matching.cu", "registration.cu", "icp.cu", "evaluation.cu", "voxel.cu", "kpconv_grad.cu", "train_ops.cu"]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]

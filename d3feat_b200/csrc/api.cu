@@ -272,6 +272,56 @@ int d3f_affine_leaky(const float* x, int N, int C, const float* scale, const flo
   return affine_leaky(x, N, C, scale, shift, residual, leaky_alpha, out, (cudaStream_t)stream, n_dev);
 }
 
+size_t d3f_batch_norm_train_workspace_bytes(int N, int C) { return batch_norm_train_workspace_bytes(N, C); }
+
+int d3f_batch_norm_train_forward(const float* x, int N, int C, const float* gamma, const float* beta,
+                                 float* moving_mean, float* moving_var, float decay, float eps, const float* residual,
+                                 float leaky_alpha, float* out, float* mean, float* invstd, void* workspace,
+                                 size_t workspace_bytes, d3f_stream_t stream) {
+  return batch_norm_train_forward(x, N, C, gamma, beta, moving_mean, moving_var, decay, eps, residual, leaky_alpha, out,
+                                  mean, invstd, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int d3f_batch_norm_train_backward(const float* x, const float* out, const float* dout, int N, int C,
+                                  const float* gamma, const float* mean, const float* invstd, float leaky_alpha,
+                                  float* dx, float* dresidual, float* dgamma, float* dbeta, void* workspace,
+                                  size_t workspace_bytes, d3f_stream_t stream) {
+  return batch_norm_train_backward(x, out, dout, N, C, gamma, mean, invstd, leaky_alpha, dx, dresidual, dgamma, dbeta,
+                                   workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t d3f_ind_max_pool_backward_workspace_bytes(int N1, int N2, int H, int C) {
+  return ind_max_pool_backward_workspace_bytes(N1, N2, H, C);
+}
+
+int d3f_ind_max_pool_backward(const float* x, const int* inds, const float* out, const float* dout, int N1, int N2,
+                              int H, int C, float* dx, void* workspace, size_t workspace_bytes, d3f_stream_t stream) {
+  return ind_max_pool_backward(x, inds, out, dout, N1, N2, H, C, dx, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t d3f_gather_rows_backward_workspace_bytes(int N1, int N2) { return gather_rows_backward_workspace_bytes(N1, N2); }
+
+int d3f_gather_rows_backward(const int* inds, const float* dout, int N1, int N2, int C, float* dx, void* workspace,
+                             size_t workspace_bytes, d3f_stream_t stream) {
+  return gather_rows_backward(inds, dout, N1, N2, C, dx, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int d3f_l2_normalize_backward(const float* x, const float* dout, int N, int C, float eps, float* dx,
+                              d3f_stream_t stream) {
+  return l2_normalize_backward(x, dout, N, C, eps, dx, (cudaStream_t)stream);
+}
+
+size_t d3f_detection_scores_backward_workspace_bytes(int N, int H, int B, int D) {
+  return detection_scores_backward_workspace_bytes(N, H, B, D);
+}
+
+int d3f_detection_scores_backward(const float* feats, const int* neighbors, const int* lengths, const float* dscores,
+                                  int B, int N, int H, int D, float* dfeats, void* workspace, size_t workspace_bytes,
+                                  d3f_stream_t stream) {
+  return detection_scores_backward(feats, neighbors, lengths, dscores, B, N, H, D, dfeats, workspace, workspace_bytes,
+                                   (cudaStream_t)stream);
+}
+
 size_t d3f_select_keypoints_workspace_bytes(int N, int B) { return select_keypoints_workspace_bytes(N, B); }
 
 int d3f_select_keypoints(const float* scores, const int* lengths, int B, int N, int k, const float* points,

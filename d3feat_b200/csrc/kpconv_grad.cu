@@ -201,6 +201,24 @@ static int grid_for(long long n, int threads = 256) {
   return (int)max(1ll, min(b, (long long)kNumSMs * 16));
 }
 
+int reverse_csr(const int* idx, int Nq, int Ns, int H, const int* nq_dev, const int* ns_dev, const SortBuffers& sb,
+                int* counts, int* offs, int* scan_scratch, const uint32_t** sorted_q, cudaStream_t stream) {
+  // a stable sort of the (q, h)-ordered entries by support gives ascending (s, q, h)
+  const int E = Nq * H;
+  D3F_CUDA(cudaMemsetAsync(counts, 0, (size_t)(Ns + 1) * sizeof(int), stream));
+  reverse_keys_kernel<<<grid_for((long long)E), 256, 0, stream>>>(idx, Nq, Ns, H, nq_dev, ns_dev, sb.keys[0],
+                                                                   sb.vals[0], counts);
+  D3F_LAUNCH_CHECK("reverse_keys_kernel");
+  int nbits = 1;
+  while (nbits < 31 && (1 << nbits) <= Ns) ++nbits;   // keys are in [0, Ns]
+  const int cur = radix_sort_pairs(sb, E, nbits, stream);
+  if (cur < 0) return cur;
+  const int rc = exclusive_scan_i32(counts, offs, Ns + 1, nullptr, scan_scratch, stream);   // counts[Ns] = 0
+  if (rc) return rc;
+  *sorted_q = sb.vals[cur];
+  return D3F_OK;
+}
+
 static int wgrad_blocks(int rows) { return rows > 0 ? ceil_div(rows, kWgRowBlock) : 1; }
 
 static int launch_wgrad_partial(const float* A, const float* B, int R, int M, int N, const int* r_dev, int r_off,
@@ -338,28 +356,20 @@ int kpconv_backward(const float* q, const float* s, const int* idx, const float*
   D3F_LAUNCH_CHECK("grad_rowscale_kernel");
 
   if (dfeat != nullptr && Hr > 0 && H > 0) {
-    // reverse table, ascending (s, q, h): a stable sort of the (q, h)-ordered entries by support
     int* counts = reinterpret_cast<int*>(reg + L.counts);
     int* offs = reinterpret_cast<int*>(reg + L.offs);
     int* rev = reinterpret_cast<int*>(ws + L.rev);
-    const int E = Nq * H;
     SortBuffers sb;
     sb.keys[0] = reinterpret_cast<uint64_t*>(reg + L.keys0);
     sb.keys[1] = reinterpret_cast<uint64_t*>(reg + L.keys1);
     sb.vals[0] = reinterpret_cast<uint32_t*>(reg + L.vals0);
     sb.vals[1] = reinterpret_cast<uint32_t*>(reg + L.vals1);
     sb.block_hist = reinterpret_cast<int*>(reg + L.hist);
-    D3F_CUDA(cudaMemsetAsync(counts, 0, (size_t)Ns * sizeof(int), stream));
-    reverse_keys_kernel<<<grid_for((long long)E), 256, 0, stream>>>(idx, Nq, Ns, H, nq_dev, ns_dev, sb.keys[0],
-                                                                     sb.vals[0], counts);
-    D3F_LAUNCH_CHECK("reverse_keys_kernel");
-    int nbits = 1;
-    while (nbits < 31 && (1 << nbits) <= Ns) ++nbits;   // keys are in [0, Ns]
-    const int cur = radix_sort_pairs(sb, E, nbits, stream);
-    if (cur < 0) return cur;
-    rc = exclusive_scan_i32(counts, offs, Ns, nullptr, reinterpret_cast<int*>(reg + L.scan), stream);
+    const uint32_t* sorted_q = nullptr;
+    rc = reverse_csr(idx, Nq, Ns, H, nq_dev, ns_dev, sb, counts, offs, reinterpret_cast<int*>(reg + L.scan), &sorted_q,
+                     stream);
     if (rc) return rc;
-    reverse_fill_kernel<<<grid_for((long long)Ns * Hr), 256, 0, stream>>>(counts, offs, sb.vals[cur], Ns, Hr, Nq, rev);
+    reverse_fill_kernel<<<grid_for((long long)Ns * Hr), 256, 0, stream>>>(counts, offs, sorted_q, Ns, Hr, Nq, rev);
     D3F_LAUNCH_CHECK("reverse_fill_kernel");
     // W^T [K, Cout, Cin] (packed for the tensor-core contraction), -Kp
     float* WT = reinterpret_cast<float*>(ws + L.WT);

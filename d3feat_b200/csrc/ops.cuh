@@ -100,6 +100,35 @@ size_t unary_backward_workspace_bytes(int N, int Cin, int Cout);
 int unary_backward(const float* x, const float* W, const float* dout, int N, int Cin, int Cout, int tensor_cores,
                    float* dx, float* dW, void* workspace, size_t workspace_bytes, cudaStream_t stream,
                    const int* n_dev);
+// Reverse neighbour table of idx[Nq, H] as a CSR, with no read-back: *sorted_q lists the query of every entry in
+// ascending (s, q, h); support s owns [offs[s], offs[s] + counts[s]). Entries that are not real (q at or past the row
+// count, idx < 0 or at or past the support count) sort last, are not counted and fill [offs[Ns], Nq * H). Sort
+// buffers for Nq * H pairs (keys[0] / vals[0] are the input), counts and offs of Ns + 1 ints, scan_scratch of
+// scan_num_blocks(Ns + 1) + 1 ints.
+struct SortBuffers;
+int reverse_csr(const int* idx, int Nq, int Ns, int H, const int* nq_dev, const int* ns_dev, const SortBuffers& sb,
+                int* counts, int* offs, int* scan_scratch, const uint32_t** sorted_q, cudaStream_t stream);
+
+// ---- train_ops.cu (training-mode batch norm; backward of the pools, l2_normalize and detection_scores) -------
+size_t batch_norm_train_workspace_bytes(int N, int C);
+int batch_norm_train_forward(const float* x, int N, int C, const float* gamma, const float* beta, float* moving_mean,
+                             float* moving_var, float decay, float eps, const float* residual, float alpha, float* out,
+                             float* mean, float* invstd, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int batch_norm_train_backward(const float* x, const float* out, const float* dout, int N, int C, const float* gamma,
+                              const float* mean, const float* invstd, float alpha, float* dx, float* dresidual,
+                              float* dgamma, float* dbeta, void* workspace, size_t workspace_bytes,
+                              cudaStream_t stream);
+size_t ind_max_pool_backward_workspace_bytes(int N1, int N2, int H, int C);
+int ind_max_pool_backward(const float* x, const int* inds, const float* out, const float* dout, int N1, int N2, int H,
+                          int C, float* dx, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+size_t gather_rows_backward_workspace_bytes(int N1, int N2);
+int gather_rows_backward(const int* inds, const float* dout, int N1, int N2, int C, float* dx, void* workspace,
+                         size_t workspace_bytes, cudaStream_t stream);
+int l2_normalize_backward(const float* x, const float* dout, int N, int C, float eps, float* dx, cudaStream_t stream);
+size_t detection_scores_backward_workspace_bytes(int N, int H, int B, int D);
+int detection_scores_backward(const float* feats, const int* neighbors, const int* lengths, const float* dscores, int B,
+                              int N, int H, int D, float* dfeats, void* workspace, size_t workspace_bytes,
+                              cudaStream_t stream);
 
 // ---- kpconv_fused.cu (one persistent kernel per layer: gather + correlation + wgmma contraction) -------
 bool kpconv_fused_supported(int Nq, int H, int K, int Cin, int Cout, int influence, int mode, const float* feat,

@@ -347,6 +347,61 @@ int d3f_affine_leaky(const float* x, int N, int C, const float* scale, const flo
                      const float* residual, float leaky_alpha, float* out, d3f_stream_t stream,
                      const int* n_dev);
 
+/* ---------------------------------------------------------------------------------------------
+ * Training (models/network_blocks.py and models/D3Feat.py with training = True, what tf.gradients gives
+ * utils/trainer.py). Exact shapes only: no device row counts. No float atomics: cross-row sums are float64 partials of
+ * fixed 2048-row blocks added in block order, a row scattered to by several outputs sums its own list (the reverse
+ * table of the indices) in ascending (q, h). Results are bitwise identical run to run and across streams. None of
+ * these synchronises.
+ *
+ * Batch norm in training mode, tf.layers.batch_normalization(training=True) on x[N,C] (unfused):
+ *   mean = sum x / N, var = sum (x - mean)^2 / N, invstd = 1/sqrt(var + eps),
+ *   out = leaky(x * gamma*invstd + (beta - mean*gamma*invstd) + residual)   (residual optional, leaky_alpha < 0: none)
+ *   moving_mean -= (moving_mean - mean) * decay, moving_var -= (moving_var - var) * decay   (decay = 1 - momentum)
+ * mean[C] and invstd[C] are written for the backward. gamma = NULL: use_batch_norm = False, out = leaky(x + beta +
+ * residual) with no statistics (moving_*, mean, invstd unused). N = 0: nothing is written, the moving statistics stay
+ * (TF would write NaN into them).
+ * Backward (dout[N,C], the forward's out): dz = dout * LeakyReluGrad (out > 0), dbeta = sum dz, dgamma = sum dz*xhat,
+ * dx = gamma*invstd*(dz - dbeta/N - xhat*dgamma/N) (gamma = NULL: dx = dz), dresidual = dz. Any output may be NULL;
+ * N = 0 gives dgamma = dbeta = 0. Workspace of both: d3f_batch_norm_train_workspace_bytes(N, C). */
+size_t d3f_batch_norm_train_workspace_bytes(int N, int C);
+int d3f_batch_norm_train_forward(const float* x, int N, int C, const float* gamma, const float* beta,
+                                 float* moving_mean, float* moving_var, float decay, float eps, const float* residual,
+                                 float leaky_alpha, float* out, float* mean, float* invstd, void* workspace,
+                                 size_t workspace_bytes, d3f_stream_t stream);
+int d3f_batch_norm_train_backward(const float* x, const float* out, const float* dout, int N, int C,
+                                  const float* gamma, const float* mean, const float* invstd, float leaky_alpha,
+                                  float* dx, float* dresidual, float* dgamma, float* dbeta, void* workspace,
+                                  size_t workspace_bytes, d3f_stream_t stream);
+
+/* Gradient of d3f_ind_max_pool (TF: reduce_max over h of gather(x || colmin(x), inds)), given its output out[N2,C]:
+ * every entry equal to out[q,c] gets dout[q,c] / (number of such entries among the H of (q, c)); an entry whose index
+ * is not in [0, N1) is the shadow row, valued colmin(x); the shadow's shares are summed and split evenly among the rows
+ * of x equal to the column minimum (reduce_min's gradient). dx[N1,C]. */
+size_t d3f_ind_max_pool_backward_workspace_bytes(int N1, int N2, int H, int C);
+int d3f_ind_max_pool_backward(const float* x, const int* inds, const float* out, const float* dout, int N1, int N2,
+                              int H, int C, float* dx, void* workspace, size_t workspace_bytes, d3f_stream_t stream);
+
+/* Gradient of a row gather out[q] = x'[inds[q]], x' = x || zeros (d3f_closest_pool on its first index column, and
+ * tf.gather): dx[s,c] = sum of dout[q,c] over the q with inds[q] == s, ascending q, rounded once. inds[N2] is one
+ * contiguous column; entries outside [0, N1) are the shadow, whose gradient is dropped. */
+size_t d3f_gather_rows_backward_workspace_bytes(int N1, int N2);
+int d3f_gather_rows_backward(const int* inds, const float* dout, int N1, int N2, int C, float* dx, void* workspace,
+                             size_t workspace_bytes, d3f_stream_t stream);
+
+/* Gradient of d3f_l2_normalize, s = sum x^2 per row: s >= eps: dx = (dout - y (y.dout)) / sqrt(s), else
+ * dx = dout / sqrt(eps). Needs no workspace. */
+int d3f_l2_normalize_backward(const float* x, const float* dout, int N, int C, float eps, float* dx,
+                              d3f_stream_t stream);
+
+/* Gradient of d3f_detection_scores for dscores[N]: ties of the channel maxima and of each cloud's maximum split
+ * evenly (reduce_max), the neighbour count is held constant (count_nonzero), softplus' = sigmoid. Rows of no cloud
+ * pass no gradient; the gradient reaching the shadow row is dropped. dfeats[N,D]. */
+size_t d3f_detection_scores_backward_workspace_bytes(int N, int H, int B, int D);
+int d3f_detection_scores_backward(const float* feats, const int* neighbors, const int* lengths, const float* dscores,
+                                  int B, int N, int H, int D, float* dfeats, void* workspace, size_t workspace_bytes,
+                                  d3f_stream_t stream);
+
 /* Keypoint selection by detection score for B stacked clouds (utils/tester.py:209-213, the 3DMatch tester: every
  * point in ascending score order; :281-290, the KITTI tester: the top k per cloud, ascending).
  *   scores[N] (N = capacity with n_dev), lengths[B] (device), optional points[N,3] and descriptors[N,D].
