@@ -73,6 +73,14 @@ SYMBOLS = [
                                 _P]),
     ("d3f_icp_pairs_workspace_bytes", _Z, [_I, _I, _I, _D, _P]),
     ("d3f_icp_pairs", _I, [_P, _P, _I, _I, _P, _P, _P, _I, _P, _D, _I, _D, _D, _P, _P, _P, _P, _P, _P, _Z, _P]),
+    ("d3f_pair_correspondences_workspace_bytes", _Z, [_I, _I, _I, _D, _P]),
+    ("d3f_pair_correspondences_count", _I, [_P, _P, _I, _I, _P, _P, _I, _P, _D, _I, _P, _P, _P, _P, _Z, _P]),
+    ("d3f_pair_correspondences_fill", _I, [_P, _I, _I, _P, _P, _I, _P, _D, _I, _I, _P, _P, _Z, _P]),
+    ("d3f_sample_correspondences_workspace_bytes", _Z, [_I, _I]),
+    ("d3f_sample_correspondences", _I, [_P, _P, _I, _I, _P, _I, _I, _I, _U64, _P, _P, _P, _P, _Z, _P]),
+    ("d3f_augment_pairs_workspace_bytes", _Z, [_I, _I]),
+    ("d3f_augment_pairs", _I, [_P, _P, _I, _I, _P, _I, _P, _U64, _D, _I, _I, _D, _D, _D, _I, _P, _P, _P, _P, _P, _P, _P,
+                               _P, _Z, _P]),
     ("d3f_evaluate_pairs_workspace_bytes", _Z, [_I, _I]),
     ("d3f_evaluate_pairs", _I, [_P, _P, _I, _I, _P, _P, _I, _P, _I, _P, _P, _P, _P, _I, _P, _I, _D, _D, _D, _D, _D, _D,
                                 _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _Z, _P]),

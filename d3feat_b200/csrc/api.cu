@@ -383,4 +383,44 @@ int d3f_evaluate_pairs(const float* points, const int* count, int B, int k, cons
                         success, recall_hit, totals, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
+size_t d3f_pair_correspondences_workspace_bytes(int N, int B, int P, double distance, const float* host_bbox) {
+  return pair_correspondences_workspace_bytes(N, B, P, distance, host_bbox);
+}
+
+int d3f_pair_correspondences_count(const float* points, const int* lengths, int B, int N, const float* host_bbox,
+                                   const int* pairs, int P, const double* trans, double distance, int mode,
+                                   long long* offset, int* count, double* overlap, void* workspace,
+                                   size_t workspace_bytes, d3f_stream_t stream) {
+  return pair_correspondences_count(points, lengths, B, N, host_bbox, pairs, P, trans, distance, mode, offset, count,
+                                    overlap, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int d3f_pair_correspondences_fill(const float* points, int B, int N, const float* host_bbox, const int* pairs, int P,
+                                  const double* trans, double distance, int mode, int M, int* rows, void* workspace,
+                                  size_t workspace_bytes, d3f_stream_t stream) {
+  return pair_correspondences_fill(points, B, N, host_bbox, pairs, P, trans, distance, mode, M, rows, workspace,
+                                   workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t d3f_sample_correspondences_workspace_bytes(int M, int P) { return sample_correspondences_workspace_bytes(M, P); }
+
+int d3f_sample_correspondences(const long long* offset, const int* rows, int M, int P, const int* anchor_len, int k,
+                               int replace, int min_count, unsigned long long seed, int* anc, int* pos, int* valid,
+                               void* workspace, size_t workspace_bytes, d3f_stream_t stream) {
+  return sample_correspondences(offset, rows, M, P, anchor_len, k, replace, min_count, seed, anc, pos, valid,
+                                workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t d3f_augment_pairs_workspace_bytes(int B, int P) { return augment_pairs_workspace_bytes(B, P); }
+
+int d3f_augment_pairs(const float* points, const int* lengths, int B, int N, const int* pairs, int P,
+                      const double* trans, unsigned long long seed, double noise, int num_axis, int scale_shift,
+                      double scale_min, double scale_max, double shift_range, int capacity, float* out_points,
+                      float* backup_points, int* out_lengths, long long* row_offset, float* R, double* scale,
+                      double* shift, void* workspace, size_t workspace_bytes, d3f_stream_t stream) {
+  return augment_pairs(points, lengths, B, N, pairs, P, trans, seed, noise, num_axis, scale_shift, scale_min, scale_max,
+                       shift_range, capacity, out_points, backup_points, out_lengths, row_offset, R, scale, shift,
+                       workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
 }  // extern "C"

@@ -1,5 +1,6 @@
-// The hash grid of neighbors.cu (cell edge = radius * 1.001, one dense cell table per cloud) and the fp64 nearest
-// query over it that ICP uses (icp.cu). The radius queries live in neighbors.cu.
+// The hash grid of neighbors.cu (cell edge = radius * 1.001, one dense cell table per cloud) and the fp64 queries
+// over it that ICP (icp.cu) and the training-pair correspondences (correspond.cu) use. The fp32 radius queries live
+// in neighbors.cu.
 #pragma once
 #include <math.h>
 
@@ -66,17 +67,18 @@ struct NbView {
   const int* cell_start;
 };
 
-// ---- nearest support of one cloud to an fp64 query ------------------------------------------------------------
+// ---- the rows of one cloud around an fp64 query ---------------------------------------------------------------
 // The query q is fp64 (a transformed fp32 point); d^2 = (e_0^2 + e_1^2) + e_2^2 with e_a = q_a - s_a, one rounding per
-// operation, as residual2 in solver.cuh. The nearest row is the one with the smallest d^2 < tau2, ties to the smaller
-// row; a NaN d^2 never qualifies.
+// operation, as residual2 in solver.cuh. visit_cloud_rows calls f(row, d^2) for every row of cloud b in the 27 cells
+// around the cell of (float)q; the callers keep the rows with d^2 < tau2 (a NaN d^2 never qualifies). The nearest row
+// (nearest_in_cloud) is the one with the smallest d^2 < tau2, ties to the smaller row.
 //
-// Why the 27 cells around the cell of (float)q hold every row with d^2 < tau2 (tau2 = tau * tau, grid radius
-// r >= tau as an fp32, cell edge c = fl(r * 1.001f)): along one axis the cell index is
+// Why the 27 cells around the cell of (float)q hold every row with d^2 < tau2 -- all of them, not only the nearest
+// (tau2 = tau * tau, grid radius r >= tau as an fp32, cell edge c = fl(r * 1.001f)): along one axis the cell index is
 //   idx(x) = clamp(floor(fl(fl(fl32(x) - mn) * inv)), 0, n - 1),   inv = fl(1 / c),
 // a composition of monotone maps (round to fp32, subtract / multiply by positive constants with round to nearest,
-// floor, clamp), so it is monotone in the real x. A row s with d^2 < tau2 has |q_a - s_a| <= tau (1 + 2^-50) on every
-// axis, so idx(s_a) lies between idx(q_a - tau') and idx(q_a + tau'); the scan is conservative when any two reals
+// floor, clamp), so it is monotone in the real x. Every row s with d^2 < tau2 has |q_a - s_a| <= tau (1 + 2^-50) on
+// every axis, so idx(s_a) lies between idx(q_a - tau') and idx(q_a + tau'); the scan is conservative when any two reals
 // a < b with b - a <= tau' get indices at most one apart. Exactly, (b - a) * inv <= tau' / (r * 1.001 (1 - 2^-24))
 // (1 + 2^-24) < 0.999002 cells, leaving a margin of 9.98e-4 cells for the roundings. If every bbox coordinate lies
 // within M = 1024 cells of the origin (checked on the host, nearest_lookup_exact), a point x within two cells of the
@@ -85,7 +87,7 @@ struct NbView {
 // most one. A point more than two cells outside the box pins, with the other point (within one cell of it), both
 // indices to the same edge cell or to the edge cell and its neighbour (monotonicity, and fl(...) of a point one cell
 // outside the box is within 1e-3 of its exact value), so the clamp keeps them within one. Non-finite queries have no
-// nearest row and are not looked up; a query beyond the fp32 range rounds to +-inf and clamps to an edge cell.
+// row within tau and are not looked up; a query beyond the fp32 range rounds to +-inf and clamps to an edge cell.
 static inline bool nearest_lookup_exact(const NbGrid& g, const float* host_bbox) {
   for (int a = 0; a < 3; ++a) {
     const double m = fmax(fabs((double)host_bbox[a]), fabs((double)host_bbox[3 + a]));
@@ -99,6 +101,33 @@ struct Nearest {
   double d2;     // tau2 when there is none
 };
 
+template <typename F>
+__device__ __forceinline__ void visit_cloud_rows(const NbView& v, int b, double q0, double q1, double q2, F&& f) {
+  const double q[3] = {q0, q1, q2};
+  if (isfinite(q0) && isfinite(q1) && isfinite(q2)) {
+    const NbGrid& g = v.g;
+    const int cx = cell_coord((float)q[0], g.minx, g.inv_cell, g.nx);
+    const int cy = cell_coord((float)q[1], g.miny, g.inv_cell, g.ny);
+    const int cz = cell_coord((float)q[2], g.minz, g.inv_cell, g.nz);
+    const int x0 = max(cx - 1, 0), x1 = min(cx + 1, g.nx - 1);
+    for (int zz = max(cz - 1, 0); zz <= min(cz + 1, g.nz - 1); ++zz) {
+      for (int yy = max(cy - 1, 0); yy <= min(cy + 1, g.ny - 1); ++yy) {
+        // cells x0..x1 of one (y, z) row are adjacent in the table: one contiguous run of sorted_pts
+        const int row = b * (int)g.ncells + (zz * g.ny + yy) * g.nx;
+        const int e = __ldg(v.cell_start + row + x1 + 1);
+        for (int i = __ldg(v.cell_start + row + x0); i < e; ++i) {
+          const float4 s = __ldg(v.sorted_pts + i);
+          const double e0 = __dsub_rn(q[0], (double)s.x), e1 = __dsub_rn(q[1], (double)s.y);
+          const double e2 = __dsub_rn(q[2], (double)s.z);
+          const double d2 = __dadd_rn(__dadd_rn(__dmul_rn(e0, e0), __dmul_rn(e1, e1)), __dmul_rn(e2, e2));
+          f((int)__float_as_uint(s.w), d2);
+        }
+      }
+    }
+  }
+}
+
+// nearest_in_cloud walks the cells itself: written over visit_cloud_rows, ICP's correspond kernel takes a stack frame
 __device__ __forceinline__ Nearest nearest_in_cloud(const NbView& v, int b, double q0, double q1, double q2,
                                                     double tau2) {
   const double q[3] = {q0, q1, q2};

@@ -179,6 +179,26 @@ int icp_pairs(const float* points, const int* lengths, int B, int N, const int* 
               double relative_fitness, double relative_rmse, double* pose, double* fitness, double* inlier_rmse,
               int* n_corr, int* iterations, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
+// ---- correspond.cu (training pairs: correspondences, keypoint sampling, augmentation) ----------------------
+size_t pair_correspondences_workspace_bytes(int N, int B, int P, double distance, const float* host_bbox);
+int pair_correspondences_count(const float* points, const int* lengths, int B, int N, const float* host_bbox,
+                               const int* pairs, int P, const double* trans, double distance, int mode,
+                               long long* offset, int* count, double* overlap, void* workspace,
+                               size_t workspace_bytes, cudaStream_t stream);
+int pair_correspondences_fill(const float* points, int B, int N, const float* host_bbox, const int* pairs, int P,
+                              const double* trans, double distance, int mode, int M, int* rows, void* workspace,
+                              size_t workspace_bytes, cudaStream_t stream);
+size_t sample_correspondences_workspace_bytes(int M, int P);
+int sample_correspondences(const long long* offset, const int* rows, int M, int P, const int* anchor_len, int k,
+                           int replace, int min_count, unsigned long long seed, int* anc, int* pos, int* valid,
+                           void* workspace, size_t workspace_bytes, cudaStream_t stream);
+size_t augment_pairs_workspace_bytes(int B, int P);
+int augment_pairs(const float* points, const int* lengths, int B, int N, const int* pairs, int P, const double* trans,
+                  unsigned long long seed, double noise, int num_axis, int scale_shift, double scale_min,
+                  double scale_max, double shift_range, int capacity, float* out_points, float* backup_points,
+                  int* out_lengths, long long* row_offset, float* R, double* scale, double* shift, void* workspace,
+                  size_t workspace_bytes, cudaStream_t stream);
+
 // ---- evaluation.cu ----------------------------------------------------------------------------------
 size_t evaluate_pairs_workspace_bytes(int P, int S);
 int evaluate_pairs(const float* points, const int* count, int B, int k, const int* matches, const int* n_matches,

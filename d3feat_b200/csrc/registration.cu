@@ -25,6 +25,7 @@
 #include <cmath>
 
 #include "ops.cuh"
+#include "rng.cuh"
 #include "solver.cuh"
 
 namespace d3f {
@@ -37,18 +38,6 @@ constexpr int kFinalizeThreads = 256;
 constexpr int kWarpsPerCta = 8;          // prepare / select: one warp per pair
 constexpr int kSelectWords = 8;          // validation words per lane and select iteration
 constexpr int kFirstRound = 8192;        // hypotheses per pair in the first round; each later round is twice as long
-
-__device__ __forceinline__ unsigned long long splitmix64(unsigned long long z) {
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
-__device__ __forceinline__ int sample_index(int p, int h, int m, int n_c, unsigned long long seed) {
-  const unsigned long long c = ((((unsigned long long)(unsigned)p) << 32) | (unsigned)h) * 8ull + (unsigned)m;
-  const unsigned long long z = splitmix64(seed + c * 0x9E3779B97F4A7C15ull);
-  return (int)(((z >> 32) * (unsigned long long)(unsigned)n_c) >> 32);
-}
 
 // the source and target point of correspondence row r of pair p (the row was validated by reg_prepare_kernel)
 struct Rows {

@@ -38,6 +38,8 @@ L2_EPSILON = 1e-10       # tf.nn.l2_normalize default (models/D3Feat.py:65)
 # training_3DMatch.py:79-113 (weights_decay: utils/config.py:137)
 TRAINING_3DMATCH = dict(batch_norm_momentum=0.98, learning_rate=1e-1, momentum=0.98, grad_clip_norm=100.0,
                         weights_decay=1e-6, det_loss_weight=1.0, safe_radius=0.1, keypts_num=256)
+# training_KITTI.py:63-113
+TRAINING_KITTI = dict(TRAINING_3DMATCH, first_subsampling_dl=0.30, safe_radius=1.0, keypts_num=1024)
 
 TRAINABLE = ("weights", "gamma", "beta", "offset")
 

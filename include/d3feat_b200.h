@@ -37,6 +37,11 @@
  *                             demo_registration.py:184-192 (Open3D's RANSAC over the keypoint correspondences,
  *                             with the edge-length and distance checkers)
  *   d3f_icp_pairs             datasets/KITTI.py:284-301 (Open3D's point-to-point registration_icp)
+ *   d3f_pair_correspondences_* datasets/KITTI.py:35-48,319-327 (get_matching_indices), datasets/cal_overlap.py:78-126
+ *                             (the BFMatcher overlap table of 3DMatch's training pairs)
+ *   d3f_sample_correspondences datasets/KITTI.py:184-189, datasets/ThreeDMatch.py:218-229 (the keypoint draw)
+ *   d3f_augment_pairs         datasets/ThreeDMatch.py:24-45,266-273, datasets/KITTI.py:191-206 (noise, rotate, scale,
+ *                             shift; the backup points the loss measures on)
  *   d3f_evaluate_pairs        geometric_registration/evaluate.py:67-82,207, repeatability/evaluate_3dmatch_our.py:30-41,
  *                             evaluate_kitti_our.py:12-23, utils/tester.py:326-342, 3dmatch/evaluate.m with
  *                             mrEvaluateRegistration.m (FMR, repeatability, RTE / RRE, registration recall)
@@ -550,6 +555,68 @@ int d3f_evaluate_pairs(const float* points, const int* count, int B, int k, cons
                        int* n_repeated, double* repeatability, double* rte, double* rre_deg, double* rmse2,
                        int* success, int* recall_hit, double* totals, void* workspace, size_t workspace_bytes,
                        d3f_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Training pairs (datasets/KITTI.py and datasets/ThreeDMatch.py's generators, datasets/cal_overlap.py). Contract:
+ * oracle/pairs_np.py, exactly. points[N,3] fp32 and lengths[B] (device, B in [1, 1024]) stacked as in d3f_icp_pairs;
+ * pairs[P,2] (device) = (anchor cloud, positive cloud), P in [1, 2^24]; trans[P,4,4] (device, fp64, row-major) maps
+ * anchor points onto the positive (GroundTruth.pose's convention). A pair naming a cloud outside [0, B) reads neither.
+ *
+ * Correspondences. Anchor row s becomes q = R s + t (fp64, one rounding per operation in d3f_icp_pairs' order, no
+ * fused multiply-add); d^2 = ((e_0^2 + e_1^2) + e_2^2) against the widened positive rows, tau^2 = distance * distance.
+ *   mode D3F_CORR_RADIUS: every positive row with d^2 < tau^2 (strict); D3F_CORR_NEAREST: the row with the smallest
+ *   d^2 < tau^2, ties to the smaller row. A non-finite q matches nothing.
+ *   d3f_pair_correspondences_count  builds the grid over the clouds in `workspace` and writes offset[P+1] (int64):
+ *                                   pair p's rows are [offset[p], offset[p+1]); count[P] (int32, saturating) and
+ *                                   overlap[P] = count / anchor rows (fp64, 0 for an empty anchor). The caller reads
+ *                                   M = offset[P] back to size `rows`.
+ *   d3f_pair_correspondences_fill   with the same arguments and workspace, after the count: rows[M,2] int32 =
+ *                                   (anchor row, positive row), cloud-local, ascending in (anchor, positive) per pair.
+ *   Limits: N >= 0; P * ceil(N / 256) * 256 within int32; distance finite and > 0; the grid (cell distance rounded
+ *   up to fp32, * 1.001) within 2^27 cells over all clouds and 4096 per axis, and every host_bbox coordinate within 1024
+ *   cells of the origin; otherwise, or for a null pointer, D3F_ERR_INVALID before any CUDA call (the workspace query
+ *   returns 0).
+ * Sampling, d3f_sample_correspondences: pair p's candidates are rows [offset[p], offset[p+1]) of rows[M,2] (offset
+ *   nondecreasing from 0 to M, as the count writes it; any other table gives an unspecified but in-bounds sample),
+ *   n = their number. valid[p] = n >= max(min_count, 1), and without replacement n >= k. replace = 1: draw m is
+ *   ((z >> 32) * n) >> 32 of its counter; replace = 0: the k candidates with the smallest (32-bit key, candidate), in
+ *   that order. anc[P,k] = the anchor row, pos[P,k] = the positive row + anchor_len[p] (device int32 [P]), -1 for an
+ *   invalid pair. Never synchronises.
+ * Augmentation, d3f_augment_pairs: for every pair and each of its two clouds (side 0: anchor, 1: positive), from the
+ *   fp32 row widened to fp64, one rounding per operation: x += u * noise per axis; num_axis (1 or 3) rotations
+ *   x_j = ((x_0 R_0j + x_1 R_1j) + x_2 R_2j) by the reference's float32 R (theta = (u * 2) * pi, R from fp64 cos / sin
+ *   rounded to fp32, row and column `axis` those of the identity; axis = floor(3 u') for num_axis = 1, 0, 1, 2 for 3);
+ *   with scale_shift: x = scale * x + shift, scale = scale_min + (scale_max - scale_min) u per pair and
+ *   shift_a = -shift_range + (2 shift_range) u per cloud; then one rounding to fp32. Outputs: out_points and
+ *   backup_points [capacity,3] (pair p's anchor then positive rows from row_offset[p]; backup = fp32 of q = trans s for
+ *   the anchor, the point itself for the positive; rows at or past min(row_offset[P], capacity) are not written),
+ *   out_lengths[P,2], row_offset[P+1] (int64), R[2P,num_axis,3,3] fp32, scale[P] and shift[2P,3] fp64 (1 and 0 without
+ *   scale_shift). Never synchronises.
+ * Counters: every draw is z = splitmix64(seed + c * 0x9E3779B97F4A7C15), c = (pair << 36) | (index << 4) | slot, and
+ *   u = (z >> 11) * 2^-53. Slots: 0-5 noise (3 * side + axis; index = cloud-local row), 6-7 rotation angle (+ side;
+ *   index = rotation), 8-9 rotation axis (+ side), 10 scale, 11-12 shift (+ side; index = axis), 13 draw with
+ *   replacement (index = m), 14 key without replacement (index = candidate; key = z >> 32).
+ * ------------------------------------------------------------------------------------------- */
+#define D3F_CORR_RADIUS 0
+#define D3F_CORR_NEAREST 1
+size_t d3f_pair_correspondences_workspace_bytes(int N, int B, int P, double distance, const float* host_bbox);
+int d3f_pair_correspondences_count(const float* points, const int* lengths, int B, int N, const float* host_bbox,
+                                   const int* pairs, int P, const double* trans, double distance, int mode,
+                                   long long* offset, int* count, double* overlap, void* workspace,
+                                   size_t workspace_bytes, d3f_stream_t stream);
+int d3f_pair_correspondences_fill(const float* points, int B, int N, const float* host_bbox, const int* pairs, int P,
+                                  const double* trans, double distance, int mode, int M, int* rows, void* workspace,
+                                  size_t workspace_bytes, d3f_stream_t stream);
+size_t d3f_sample_correspondences_workspace_bytes(int M, int P);
+int d3f_sample_correspondences(const long long* offset, const int* rows, int M, int P, const int* anchor_len, int k,
+                               int replace, int min_count, unsigned long long seed, int* anc, int* pos, int* valid,
+                               void* workspace, size_t workspace_bytes, d3f_stream_t stream);
+size_t d3f_augment_pairs_workspace_bytes(int B, int P);
+int d3f_augment_pairs(const float* points, const int* lengths, int B, int N, const int* pairs, int P,
+                      const double* trans, unsigned long long seed, double noise, int num_axis, int scale_shift,
+                      double scale_min, double scale_max, double shift_range, int capacity, float* out_points,
+                      float* backup_points, int* out_lengths, long long* row_offset, float* R, double* scale,
+                      double* shift, void* workspace, size_t workspace_bytes, d3f_stream_t stream);
 
 #ifdef __cplusplus
 }
