@@ -295,7 +295,7 @@ bool corr_args_ok(int N, int B, int P, double distance, const float* host_bbox) 
 // every size the workspace depends on, or 0
 size_t corr_layout(int N, int B, int P, double distance, const float* host_bbox, CorrWork* w, void* base) {
   if (!corr_args_ok(N, B, P, distance, host_bbox)) return 0;
-  const size_t nb = radius_neighbors_workspace_bytes(N, B, grid_radius(distance), host_bbox);
+  const size_t nb = d3f_radius_neighbors_workspace_bytes(N, B, grid_radius(distance), host_bbox);
   if (nb == 0) return 0;
   Carver cv(base, ~(size_t)0);
   CorrWork x;
@@ -526,17 +526,23 @@ size_t aug_layout(int B, int P, int** start, int4** info, void* base) {
 }
 
 }  // namespace
+}  // namespace d3f
 
 // ---- host entry points -------------------------------------------------------------------------------------------
 
-size_t pair_correspondences_workspace_bytes(int N, int B, int P, double distance, const float* host_bbox) {
+using namespace d3f;
+
+extern "C" size_t d3f_pair_correspondences_workspace_bytes(int N, int B, int P, double distance,
+                                                           const float* host_bbox) {
   return corr_layout(N, B, P, distance, host_bbox, nullptr, nullptr);
 }
 
-int pair_correspondences_count(const float* points, const int* lengths, int B, int N, const float* host_bbox,
-                               const int* pairs, int P, const double* trans, double distance, int mode,
-                               long long* offset, int* count, double* overlap, void* workspace,
-                               size_t workspace_bytes, cudaStream_t stream) {
+extern "C" int d3f_pair_correspondences_count(const float* points, const int* lengths, int B, int N,
+                                              const float* host_bbox, const int* pairs, int P, const double* trans,
+                                              double distance, int mode, long long* offset, int* count,
+                                              double* overlap, void* workspace, size_t workspace_bytes,
+                                              d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   const char* who = "pair_correspondences_count";
   CorrWork w;
   int rc = corr_check(who, points, B, N, host_bbox, pairs, P, trans, distance, mode, workspace, workspace_bytes, &w);
@@ -564,9 +570,11 @@ int pair_correspondences_count(const float* points, const int* lengths, int B, i
   return D3F_OK;
 }
 
-int pair_correspondences_fill(const float* points, int B, int N, const float* host_bbox, const int* pairs, int P,
-                              const double* trans, double distance, int mode, int M, int* rows, void* workspace,
-                              size_t workspace_bytes, cudaStream_t stream) {
+extern "C" int d3f_pair_correspondences_fill(const float* points, int B, int N, const float* host_bbox,
+                                             const int* pairs, int P, const double* trans, double distance, int mode,
+                                             int M, int* rows, void* workspace, size_t workspace_bytes,
+                                             d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   const char* who = "pair_correspondences_fill";
   CorrWork w;
   int rc = corr_check(who, points, B, N, host_bbox, pairs, P, trans, distance, mode, workspace, workspace_bytes, &w);
@@ -585,11 +593,15 @@ int pair_correspondences_fill(const float* points, int B, int N, const float* ho
   return D3F_OK;
 }
 
-size_t sample_correspondences_workspace_bytes(int M, int P) { return sample_layout(M, P, nullptr, nullptr); }
+extern "C" size_t d3f_sample_correspondences_workspace_bytes(int M, int P) {
+  return sample_layout(M, P, nullptr, nullptr);
+}
 
-int sample_correspondences(const long long* offset, const int* rows, int M, int P, const int* anchor_len, int k,
-                           int replace, int min_count, unsigned long long seed, int* anc, int* pos, int* valid,
-                           void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+extern "C" int d3f_sample_correspondences(const long long* offset, const int* rows, int M, int P, const int* anchor_len,
+                                          int k, int replace, int min_count, unsigned long long seed, int* anc,
+                                          int* pos, int* valid, void* workspace, size_t workspace_bytes,
+                                          d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   const char* who = "sample_correspondences";
   D3F_REQUIRE(M >= 0 && P >= 1 && P <= kMaxPairs && k >= 1 && (long long)P * k <= INT32_MAX, D3F_ERR_INVALID,
               "%s: bad shape M=%d P=%d k=%d", who, M, P, k);
@@ -615,13 +627,17 @@ int sample_correspondences(const long long* offset, const int* rows, int M, int 
   return D3F_OK;
 }
 
-size_t augment_pairs_workspace_bytes(int B, int P) { return aug_layout(B, P, nullptr, nullptr, nullptr); }
+extern "C" size_t d3f_augment_pairs_workspace_bytes(int B, int P) {
+  return aug_layout(B, P, nullptr, nullptr, nullptr);
+}
 
-int augment_pairs(const float* points, const int* lengths, int B, int N, const int* pairs, int P, const double* trans,
-                  unsigned long long seed, double noise, int num_axis, int scale_shift, double scale_min,
-                  double scale_max, double shift_range, int capacity, float* out_points, float* backup_points,
-                  int* out_lengths, long long* row_offset, float* R, double* scale, double* shift, void* workspace,
-                  size_t workspace_bytes, cudaStream_t stream) {
+extern "C" int d3f_augment_pairs(const float* points, const int* lengths, int B, int N, const int* pairs, int P,
+                                 const double* trans, unsigned long long seed, double noise, int num_axis,
+                                 int scale_shift, double scale_min, double scale_max, double shift_range, int capacity,
+                                 float* out_points, float* backup_points, int* out_lengths, long long* row_offset,
+                                 float* R, double* scale, double* shift, void* workspace, size_t workspace_bytes,
+                                 d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   const char* who = "augment_pairs";
   D3F_REQUIRE(B >= 1 && B <= kMaxBatch, D3F_ERR_INVALID, "%s: B=%d must be in [1,%d]", who, B, kMaxBatch);
   D3F_REQUIRE(N >= 0 && P >= 1 && P <= kMaxPairs && capacity >= 0, D3F_ERR_INVALID,
@@ -652,5 +668,3 @@ int augment_pairs(const float* points, const int* lengths, int B, int N, const i
   D3F_LAUNCH_CHECK("aug_points_kernel");
   return D3F_OK;
 }
-
-}  // namespace d3f

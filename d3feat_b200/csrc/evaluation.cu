@@ -329,19 +329,25 @@ eval_totals_kernel(int P, const __grid_constant__ EvalParams prm, Outputs o) {
 bool finite_positive(double x) { return std::isfinite(x) && x > 0.0; }
 
 }  // namespace
+}  // namespace d3f
 
-size_t evaluate_pairs_workspace_bytes(int P, int S) {
+using namespace d3f;
+
+extern "C" size_t d3f_evaluate_pairs_workspace_bytes(int P, int S) {
   if (P < 1 || S < 0 || S > kMaxPoseSets) return 0;
   return align_up(sizeof(int) * (size_t)(S > 0 ? S : 1) * P, 256);
 }
 
-int evaluate_pairs(const float* points, const int* count, int B, int k, const int* matches, const int* n_matches,
-                   int L, const int* pairs, int P, const double* truth_pose, const double* truth_info,
-                   const int* truth_flags, const double* const* poses, int S, const int* levels, int R,
-                   double fmr_distance, double fmr_ratio, double repeat_distance, double err2, double rte_max,
-                   double rre_max_deg, int* valid, int* n_match_inliers, double* inlier_ratio, int* fmr_hit,
-                   int* n_repeated, double* repeatability, double* rte, double* rre_deg, double* rmse2, int* success,
-                   int* recall_hit, double* totals, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+extern "C" int d3f_evaluate_pairs(const float* points, const int* count, int B, int k, const int* matches,
+                                  const int* n_matches, int L, const int* pairs, int P, const double* truth_pose,
+                                  const double* truth_info, const int* truth_flags, const double* const* poses, int S,
+                                  const int* levels, int R, double fmr_distance, double fmr_ratio,
+                                  double repeat_distance, double err2, double rte_max, double rre_max_deg, int* valid,
+                                  int* n_match_inliers, double* inlier_ratio, int* fmr_hit, int* n_repeated,
+                                  double* repeatability, double* rte, double* rre_deg, double* rmse2, int* success,
+                                  int* recall_hit, double* totals, void* workspace, size_t workspace_bytes,
+                                  d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(B >= 1 && B <= kMaxBatch, D3F_ERR_INVALID, "evaluate_pairs: B=%d must be in [1,%d]", B, kMaxBatch);
   D3F_REQUIRE(k >= 1 && L >= 1 && P >= 1, D3F_ERR_INVALID, "evaluate_pairs: bad shape k=%d L=%d P=%d", k, L, P);
   D3F_REQUIRE((long long)P * k <= INT32_MAX && (long long)P * L * 2 <= INT32_MAX && (long long)B * k * 3 <= INT32_MAX,
@@ -370,9 +376,9 @@ int evaluate_pairs(const float* points, const int* count, int B, int k, const in
               D3F_ERR_INVALID, "evaluate_pairs: null pointer");
   for (int s = 0; s < S; ++s)
     D3F_REQUIRE(poses[s] != nullptr, D3F_ERR_INVALID, "evaluate_pairs: null pointer (poses[%d])", s);
-  D3F_REQUIRE(workspace_bytes >= evaluate_pairs_workspace_bytes(P, S), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_evaluate_pairs_workspace_bytes(P, S), D3F_ERR_WORKSPACE,
               "evaluate_pairs: workspace too small (%zu < %zu bytes)", workspace_bytes,
-              evaluate_pairs_workspace_bytes(P, S));
+              d3f_evaluate_pairs_workspace_bytes(P, S));
   EvalParams prm = {};
   for (int r = 0; r < R; ++r) prm.levels[r] = levels[r];
   prm.R = R;
@@ -405,5 +411,3 @@ int evaluate_pairs(const float* points, const int* count, int B, int k, const in
   D3F_LAUNCH_CHECK("eval_totals_kernel");
   return D3F_OK;
 }
-
-}  // namespace d3f

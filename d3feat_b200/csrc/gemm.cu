@@ -170,3 +170,27 @@ int gemm_f32(const float* A, const float* B, float* C, int M, int N, int K, cons
 }
 
 }  // namespace d3f
+
+using namespace d3f;
+
+extern "C" int d3f_unary_forward(const float* x, const float* W, const float* W_packed, int N, int Cin, int Cout,
+                                 const float* bn_scale, const float* bn_shift, const float* bias, const float* residual,
+                                 float leaky_alpha, float* out, d3f_stream_t stream, const int* n_dev) {
+  D3F_REQUIRE(N >= 0 && Cin >= 1 && Cout >= 1, D3F_ERR_INVALID, "d3f_unary_forward: bad shape N=%d Cin=%d Cout=%d", N,
+              Cin, Cout);
+  D3F_REQUIRE(N == 0 || (x && W && out), D3F_ERR_INVALID, "d3f_unary_forward: null pointer");
+  D3F_REQUIRE((bn_scale == nullptr) == (bn_shift == nullptr), D3F_ERR_INVALID,
+              "d3f_unary_forward: bn_scale/bn_shift mismatch");
+  Epilogue ep;
+  ep.rowscale = nullptr;
+  ep.bn_scale = bn_scale;
+  ep.bn_shift = bn_shift;
+  ep.bias = bias;
+  ep.residual = residual;
+  ep.leaky_alpha = leaky_alpha;
+  ep.row_map = nullptr;
+  ep.m_dev = n_dev;
+  if (W_packed != nullptr && tc_gemm_supported(x, Cin))
+    return tc_gemm(x, W_packed, out, N, Cout, Cin, ep, (cudaStream_t)stream);
+  return gemm_f32(x, W, out, N, Cout, Cin, ep, (cudaStream_t)stream);
+}

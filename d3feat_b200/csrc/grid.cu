@@ -98,8 +98,15 @@ __global__ void bbox_decode_kernel(const unsigned* __restrict__ ord, float* __re
   if (i < n) out[i] = ord2f(ord[i]);
 }
 
+}  // namespace d3f
+
+using namespace d3f;
+
 // Whole-cloud bbox (B = 1) into 6 device floats. Uses out_bbox itself as the ordered-uint scratch.
-int bbox_device(const float* pts, int N, float* out_bbox, cudaStream_t stream) {
+extern "C" int d3f_bbox(const float* pts, int N, float* out_bbox, d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  D3F_REQUIRE(pts != nullptr || N == 0, D3F_ERR_INVALID, "d3f_bbox: null points");
+  D3F_REQUIRE(out_bbox != nullptr && N >= 0, D3F_ERR_INVALID, "d3f_bbox: bad arguments");
   unsigned* ord = (unsigned*)out_bbox;
   D3F_CUDA(cudaMemsetAsync(ord, 0xff, 3 * sizeof(unsigned), stream));
   D3F_CUDA(cudaMemsetAsync(ord + 3, 0, 3 * sizeof(unsigned), stream));
@@ -112,6 +119,8 @@ int bbox_device(const float* pts, int N, float* out_bbox, cudaStream_t stream) {
   D3F_LAUNCH_CHECK("bbox_decode_kernel");
   return 0;
 }
+
+namespace d3f {
 
 // ---------------------------------------------------------------------------------------------------
 // Reference grid geometry of one cloud (grid_subsampling.cpp:25-31), from its ordered-uint bbox.
@@ -282,12 +291,6 @@ static size_t carve_subsample(Carver& cv, int N, int B, SubsampleWs& w) {
   return cv.off;
 }
 
-size_t grid_subsample_workspace_bytes(int N, int B) {
-  Carver cv(nullptr, ~(size_t)0);
-  SubsampleWs w;
-  return carve_subsample(cv, N, B, w) + 256;
-}
-
 int grid_subsample(const float* pts, const int* batch_len, int B, int N, float dl, const float* feats, int fdim,
                    const int* classes, int ldim, const float* host_bbox, float* out_pts, float* out_feats,
                    int* out_classes, int* out_batch_len, int* out_M, void* workspace, size_t workspace_bytes,
@@ -298,7 +301,7 @@ int grid_subsample(const float* pts, const int* batch_len, int B, int N, float d
   D3F_REQUIRE(host_bbox != nullptr, D3F_ERR_INVALID, "grid_subsample: host_bbox is required");
   D3F_REQUIRE((feats == nullptr) == (fdim == 0) && (classes == nullptr) == (ldim == 0), D3F_ERR_INVALID,
               "grid_subsample: feats/fdim or classes/ldim mismatch");
-  D3F_REQUIRE(workspace_bytes >= grid_subsample_workspace_bytes(N, B), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_grid_subsample_workspace_bytes(N, B), D3F_ERR_WORKSPACE,
               "grid_subsample: workspace too small");
   Carver cv(workspace, workspace_bytes);
   SubsampleWs w;
@@ -362,3 +365,22 @@ int grid_subsample_error_flag(const void* workspace, size_t workspace_bytes, int
 }
 
 }  // namespace d3f
+
+extern "C" size_t d3f_grid_subsample_workspace_bytes(int N, int B) {
+  Carver cv(nullptr, ~(size_t)0);
+  SubsampleWs w;
+  return carve_subsample(cv, N, B, w) + 256;
+}
+
+extern "C" int d3f_grid_subsample(const float* pts, const int* batch_len, int B, int N, float dl, const float* feats,
+                                  int fdim, const int* classes, int ldim, const float* host_bbox, float* out_pts,
+                                  float* out_feats, int* out_classes, int* out_batch_len, int* out_M, void* workspace,
+                                  size_t workspace_bytes, d3f_stream_t stream) {
+  D3F_REQUIRE((pts != nullptr || N == 0) && batch_len != nullptr && out_pts != nullptr && out_batch_len != nullptr &&
+                  out_M != nullptr && workspace != nullptr,
+              D3F_ERR_INVALID, "d3f_grid_subsample: null pointer");
+  D3F_REQUIRE((fdim == 0 || out_feats != nullptr) && (ldim == 0 || out_classes != nullptr), D3F_ERR_INVALID,
+              "d3f_grid_subsample: missing feature / class output");
+  return grid_subsample(pts, batch_len, B, N, dl, feats, fdim, classes, ldim, host_bbox, out_pts, out_feats,
+                        out_classes, out_batch_len, out_M, workspace, workspace_bytes, (cudaStream_t)stream);
+}

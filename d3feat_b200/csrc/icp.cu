@@ -317,7 +317,7 @@ size_t workspace_layout(int N, int B, int P, double distance, const float* host_
   const float r = grid_radius(distance);
   const NbGrid g = make_grid(host_bbox, r);
   if (g.ncells * B > kMaxGridCells || !nearest_lookup_exact(g, host_bbox)) return 0;
-  const size_t nb = radius_neighbors_workspace_bytes(N, B, r, host_bbox);
+  const size_t nb = d3f_radius_neighbors_workspace_bytes(N, B, r, host_bbox);
   if (nb == 0) return 0;
   Carver cv(base, ~(size_t)0);
   Work x;
@@ -335,15 +335,20 @@ size_t workspace_layout(int N, int B, int P, double distance, const float* host_
 }
 
 }  // namespace
+}  // namespace d3f
 
-size_t icp_pairs_workspace_bytes(int N, int B, int P, double distance, const float* host_bbox) {
+using namespace d3f;
+
+extern "C" size_t d3f_icp_pairs_workspace_bytes(int N, int B, int P, double distance, const float* host_bbox) {
   return workspace_layout(N, B, P, distance, host_bbox, nullptr, nullptr);
 }
 
-int icp_pairs(const float* points, const int* lengths, int B, int N, const int* n_dev, const float* host_bbox,
-              const int* pairs, int P, const double* init, double distance, int max_iterations,
-              double relative_fitness, double relative_rmse, double* pose, double* fitness, double* inlier_rmse,
-              int* n_corr, int* iterations, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+extern "C" int d3f_icp_pairs(const float* points, const int* lengths, int B, int N, const int* n_dev,
+                             const float* host_bbox, const int* pairs, int P, const double* init, double distance,
+                             int max_iterations, double relative_fitness, double relative_rmse, double* pose,
+                             double* fitness, double* inlier_rmse, int* n_corr, int* iterations, void* workspace,
+                             size_t workspace_bytes, d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(B >= 1 && B <= kMaxBatch, D3F_ERR_INVALID, "icp_pairs: B=%d must be in [1,%d]", B, kMaxBatch);
   D3F_REQUIRE(N >= 0 && P >= 1, D3F_ERR_INVALID, "icp_pairs: bad shape N=%d P=%d", N, P);
   D3F_REQUIRE(max_iterations >= 0 && max_iterations <= 1024, D3F_ERR_INVALID,
@@ -397,5 +402,3 @@ int icp_pairs(const float* points, const int* lengths, int B, int N, const int* 
   }
   return D3F_OK;
 }
-
-}  // namespace d3f

@@ -70,16 +70,21 @@ static int keypoint_key_bits(int B) {
   return 32 + bits;
 }
 
-size_t select_keypoints_workspace_bytes(int N, int B) {
+}  // namespace d3f
+
+using namespace d3f;
+
+extern "C" size_t d3f_select_keypoints_workspace_bytes(int N, int B) {
   if (N < 0 || B < 1) return 0;
   return align_up(sizeof(int) * ((size_t)B + 1), 256) + 2 * align_up(sizeof(uint64_t) * (size_t)N, 256) +
          2 * align_up(sizeof(uint32_t) * (size_t)N, 256) + align_up(sizeof(int) * 256 * (size_t)sort_num_blocks(N), 256);
 }
 
-int select_keypoints(const float* scores, const int* lengths, int B, int N, int k, const float* points,
-                     const float* descriptors, int D, int* out_order, int* out_index, int* out_count, float* out_points,
-                     float* out_descriptors, float* out_scores, void* workspace, size_t workspace_bytes,
-                     cudaStream_t stream, const int* n_dev) {
+extern "C" int d3f_select_keypoints(const float* scores, const int* lengths, int B, int N, int k, const float* points,
+                                    const float* descriptors, int D, int* out_order, int* out_index, int* out_count,
+                                    float* out_points, float* out_descriptors, float* out_scores, void* workspace,
+                                    size_t workspace_bytes, d3f_stream_t stream_, const int* n_dev) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   const bool per_cloud = out_index || out_count || out_points || out_descriptors || out_scores;
   D3F_REQUIRE(B >= 1 && B <= kMaxBatch, D3F_ERR_INVALID, "select_keypoints: B=%d must be in [1,%d]", B, kMaxBatch);
   D3F_REQUIRE(N >= 0, D3F_ERR_INVALID, "select_keypoints: bad shape N=%d", N);
@@ -92,7 +97,7 @@ int select_keypoints(const float* scores, const int* lengths, int B, int N, int 
               "select_keypoints: gathered descriptors requested without descriptors");
   D3F_REQUIRE(lengths != nullptr && workspace != nullptr && (scores != nullptr || N == 0), D3F_ERR_INVALID,
               "select_keypoints: null pointer");
-  D3F_REQUIRE(workspace_bytes >= select_keypoints_workspace_bytes(N, B), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_select_keypoints_workspace_bytes(N, B), D3F_ERR_WORKSPACE,
               "select_keypoints: workspace too small");
   Carver cv(workspace, workspace_bytes);
   int* start = cv.take<int>((size_t)B + 1);
@@ -125,5 +130,3 @@ int select_keypoints(const float* scores, const int* lengths, int B, int N, int 
   }
   return D3F_OK;
 }
-
-}  // namespace d3f

@@ -1196,19 +1196,6 @@ int kpconv_stage1_wf(const float* q, const float4* s4, const int* idx, const flo
   return launch_stage1<false>(K, p, stream);
 }
 
-size_t kpconv_workspace_bytes(int Nq, int Ns, int H, int K, int Cin, int Cout) {
-  (void)H; (void)Cout;
-  int chunk = chunk_queries(K, Cin);
-  if (chunk > Nq) chunk = Nq > 0 ? Nq : 1;
-  size_t b = 0;
-  b += 2 * align_up((size_t)chunk * K * Cin * sizeof(float), 256);   // wf is double-buffered (stage 1 / GEMM overlap)
-  b += 2 * align_up((size_t)chunk * sizeof(float), 256);
-  b += align_up((size_t)(Ns + 1) * sizeof(float4), 256);
-  b += align_up(tc_gemm_split_ws_floats(chunk, Cout, K * Cin) * sizeof(float), 256);
-  b += align_up(kpconv_fused_workspace_bytes(), 256);
-  return b + 1024;
-}
-
 int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* idx, const float* feat,
                         const float* Kp, const float* offsets, const float* modulations, const float* W,
                         const float* W_packed, const int* query_order, int Nq, int Ns, int H, int K, int Cin, int Cout,
@@ -1227,7 +1214,7 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
   D3F_REQUIRE(extent > 0.f, D3F_ERR_INVALID, "kpconv: KP_extent=%g", (double)extent);
   D3F_REQUIRE((bn_scale == nullptr) == (bn_shift == nullptr), D3F_ERR_INVALID, "kpconv: bn_scale/bn_shift mismatch");
   D3F_REQUIRE(!deform || offsets != nullptr || Nq == 0, D3F_ERR_INVALID, "kpconv_deform: offsets missing");
-  D3F_REQUIRE(workspace_bytes >= kpconv_workspace_bytes(Nq, Ns, H, K, Cin, Cout), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_kpconv_workspace_bytes(Nq, Ns, H, K, Cin, Cout), D3F_ERR_WORKSPACE,
               "kpconv: workspace too small");
   if (Nq == 0) return D3F_OK;
   int chunk = chunk_queries(K, Cin);
@@ -1330,3 +1317,46 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
 }
 
 }  // namespace d3f
+
+using namespace d3f;
+
+extern "C" size_t d3f_kpconv_workspace_bytes(int Nq, int Ns, int H, int K, int Cin, int Cout) {
+  (void)H; (void)Cout;
+  int chunk = chunk_queries(K, Cin);
+  if (chunk > Nq) chunk = Nq > 0 ? Nq : 1;
+  size_t b = 0;
+  b += 2 * align_up((size_t)chunk * K * Cin * sizeof(float), 256);   // wf is double-buffered (stage 1 / GEMM overlap)
+  b += 2 * align_up((size_t)chunk * sizeof(float), 256);
+  b += align_up((size_t)(Ns + 1) * sizeof(float4), 256);
+  b += align_up(tc_gemm_split_ws_floats(chunk, Cout, K * Cin) * sizeof(float), 256);
+  b += align_up(kpconv_fused_workspace_bytes(), 256);
+  return b + 1024;
+}
+
+extern "C" int d3f_kpconv_forward(const float* q, const float* s, const int* idx, const float* feat, const float* Kp,
+                                  const float* W, const float* W_packed, const int* query_order, int Nq, int Ns, int H,
+                                  int K, int Cin, int Cout, float extent, int influence, int mode, int normalize,
+                                  const float* bn_scale, const float* bn_shift, const float* bias, float leaky_alpha,
+                                  float* out, void* workspace, size_t workspace_bytes, d3f_stream_t stream,
+                                  const int* nq_dev, const int* ns_dev) {
+  // an empty support set (Ns == 0: every index is the shadow point) has no coordinates or features to point at
+  D3F_REQUIRE(Nq == 0 || (q && idx && Kp && W && out && workspace && (Ns == 0 || (s && feat))), D3F_ERR_INVALID,
+              "d3f_kpconv_forward: null pointer");
+  return kpconv_forward_impl(false, q, s, idx, feat, Kp, nullptr, nullptr, W, W_packed, query_order, Nq, Ns, H, K, Cin,
+                             Cout, extent, influence, mode, normalize, bn_scale, bn_shift, bias, leaky_alpha, out,
+                             workspace, workspace_bytes, (cudaStream_t)stream, nq_dev, ns_dev);
+}
+
+extern "C" int d3f_kpconv_deform_forward(const float* q, const float* s, const int* idx, const float* feat,
+                                         const float* Kp, const float* offsets, const float* modulations,
+                                         const float* W, const float* W_packed, const int* query_order, int Nq, int Ns,
+                                         int H, int K, int Cin, int Cout, float extent, int influence, int mode,
+                                         const float* bn_scale, const float* bn_shift, const float* bias,
+                                         float leaky_alpha, float* out, void* workspace, size_t workspace_bytes,
+                                         d3f_stream_t stream, const int* nq_dev, const int* ns_dev) {
+  D3F_REQUIRE(Nq == 0 || (q && idx && Kp && W && out && workspace && offsets && (Ns == 0 || (s && feat))),
+              D3F_ERR_INVALID, "d3f_kpconv_deform_forward: null pointer");
+  return kpconv_forward_impl(true, q, s, idx, feat, Kp, offsets, modulations, W, W_packed, query_order, Nq, Ns, H, K,
+                             Cin, Cout, extent, influence, mode, 0, bn_scale, bn_shift, bias, leaky_alpha, out,
+                             workspace, workspace_bytes, (cudaStream_t)stream, nq_dev, ns_dev);
+}

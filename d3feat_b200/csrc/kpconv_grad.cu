@@ -262,7 +262,7 @@ static BackwardLayout backward_layout(int Nq, int Ns, int H, int K, int Cin, int
   L.rev = take((size_t)Ns * (Hr > 0 ? Hr : 1) * sizeof(int));
   L.nKp = take((size_t)K * 3 * sizeof(float));
   L.WT = take((size_t)K * Cout * Cin * sizeof(float));
-  L.WTp = take(tc_packed_floats(K * Cout, Cin) * sizeof(float));
+  L.WTp = take(d3f_packed_weight_floats(K * Cout, Cin) * sizeof(float));
   L.region = align_up(off, 256);
   // table build
   const long long E = (long long)Nq * H;
@@ -279,7 +279,7 @@ static BackwardLayout backward_layout(int Nq, int Ns, int H, int K, int Cin, int
   L.hist = rtake((size_t)256 * sort_num_blocks((int)E) * sizeof(int));
   const size_t build = align_up(r, 256);
   // transposed forward: Ns queries, Nq supports, Hr neighbours, Cout -> Cin channels
-  L.fwd_bytes = kpconv_workspace_bytes(Ns, Nq, Hr, K, Cout, Cin);
+  L.fwd_bytes = d3f_kpconv_workspace_bytes(Ns, Nq, Hr, K, Cout, Cin);
   // weight gradient
   L.chunk = kpconv_chunk_queries(K, Cin);
   if (L.chunk > Nq) L.chunk = Nq > 0 ? Nq : 1;
@@ -296,13 +296,19 @@ static BackwardLayout backward_layout(int Nq, int Ns, int H, int K, int Cin, int
   return L;
 }
 
-size_t kpconv_backward_workspace_bytes(int Nq, int Ns, int H, int K, int Cin, int Cout, int Hr) {
+}  // namespace d3f
+
+using namespace d3f;
+
+extern "C" size_t d3f_kpconv_backward_workspace_bytes(int Nq, int Ns, int H, int K, int Cin, int Cout, int Hr) {
   if (Nq < 0 || Ns < 0 || H < 0 || K < 1 || Cin < 1 || Cout < 1 || Hr < 0) return 0;
   return backward_layout(Nq, Ns, H, K, Cin, Cout, Hr).total;
 }
 
-int kpconv_reverse_width(const int* idx, int Nq, int Ns, int H, int* width, void* workspace, size_t workspace_bytes,
-                         cudaStream_t stream, const int* nq_dev, const int* ns_dev) {
+extern "C" int d3f_kpconv_reverse_width(const int* idx, int Nq, int Ns, int H, int* width, void* workspace,
+                                        size_t workspace_bytes, d3f_stream_t stream_, const int* nq_dev,
+                                        const int* ns_dev) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(Nq >= 0 && Ns >= 0 && H >= 0 && width != nullptr, D3F_ERR_INVALID,
               "kpconv_reverse_width: bad arguments Nq=%d Ns=%d H=%d", Nq, Ns, H);
   *width = 0;
@@ -325,10 +331,15 @@ int kpconv_reverse_width(const int* idx, int Nq, int Ns, int H, int* width, void
   return D3F_OK;
 }
 
-int kpconv_backward(const float* q, const float* s, const int* idx, const float* feat, const float* Kp, const float* W,
-                    const float* dout, int Nq, int Ns, int H, int Hr, int K, int Cin, int Cout, float extent,
-                    int influence, int mode, int normalize, int tensor_cores, float* dfeat, float* dW, void* workspace,
-                    size_t workspace_bytes, cudaStream_t stream, const int* nq_dev, const int* ns_dev) {
+extern "C" int d3f_kpconv_backward(const float* q, const float* s, const int* idx, const float* feat, const float* Kp,
+                                   const float* W, const float* dout, int Nq, int Ns, int H, int Hr, int K, int Cin,
+                                   int Cout, float extent, int influence, int mode, int normalize, int tensor_cores,
+                                   float* dfeat, float* dW, void* workspace, size_t workspace_bytes,
+                                   d3f_stream_t stream_, const int* nq_dev, const int* ns_dev) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  D3F_REQUIRE(Nq == 0 || Ns == 0 || (dfeat == nullptr && dW == nullptr) ||
+                  (q && s && idx && feat && Kp && W && dout && workspace),
+              D3F_ERR_INVALID, "d3f_kpconv_backward: null pointer");
   D3F_REQUIRE(Nq >= 0 && Ns >= 0 && H >= 0 && Hr >= 0 && Cin >= 1 && Cout >= 1, D3F_ERR_INVALID,
               "kpconv_backward: bad shape Nq=%d Ns=%d H=%d Hr=%d Cin=%d Cout=%d", Nq, Ns, H, Hr, Cin, Cout);
   D3F_REQUIRE(K >= 1 && K <= 64, D3F_ERR_INVALID, "kpconv_backward: num_kernel_points=%d outside [1, 64]", K);
@@ -381,7 +392,7 @@ int kpconv_backward(const float* q, const float* s, const int* idx, const float*
     float* WTp = nullptr;
     if (tensor_cores) {
       WTp = reinterpret_cast<float*>(ws + L.WTp);
-      rc = tc_pack_weight(WT, K * Cout, Cin, WTp, stream);
+      rc = d3f_pack_weight(WT, K * Cout, Cin, WTp, stream);
       if (rc) return rc;
     }
     rc = kpconv_forward_impl(false, s, q, rev, G, nKp, nullptr, nullptr, WT, WTp, nullptr, Ns, Nq, Hr, K, Cout, Cin,
@@ -410,27 +421,30 @@ int kpconv_backward(const float* q, const float* s, const int* idx, const float*
 }
 
 // ---- unary ----------------------------------------------------------------------------------------------------------
-size_t unary_backward_workspace_bytes(int N, int Cin, int Cout) {
+extern "C" size_t d3f_unary_backward_workspace_bytes(int N, int Cin, int Cout) {
   if (N < 0 || Cin < 1 || Cout < 1) return 0;
   size_t b = align_up((size_t)Cin * Cout * sizeof(float), 256);
-  b += align_up(tc_packed_floats(Cout, Cin) * sizeof(float), 256);
+  b += align_up(d3f_packed_weight_floats(Cout, Cin) * sizeof(float), 256);
   b += align_up((size_t)wgrad_blocks(N) * Cin * Cout * sizeof(float), 256);
   return b + 1024;
 }
 
-int unary_backward(const float* x, const float* W, const float* dout, int N, int Cin, int Cout, int tensor_cores,
-                   float* dx, float* dW, void* workspace, size_t workspace_bytes, cudaStream_t stream,
-                   const int* n_dev) {
+extern "C" int d3f_unary_backward(const float* x, const float* W, const float* dout, int N, int Cin, int Cout,
+                                  int tensor_cores, float* dx, float* dW, void* workspace, size_t workspace_bytes,
+                                  d3f_stream_t stream_, const int* n_dev) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  D3F_REQUIRE(N == 0 || (dx == nullptr && dW == nullptr) || (x && W && dout && workspace), D3F_ERR_INVALID,
+              "d3f_unary_backward: null pointer");
   D3F_REQUIRE(N >= 0 && Cin >= 1 && Cout >= 1, D3F_ERR_INVALID, "unary_backward: bad shape N=%d Cin=%d Cout=%d", N,
               Cin, Cout);
-  D3F_REQUIRE(workspace_bytes >= unary_backward_workspace_bytes(N, Cin, Cout), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_unary_backward_workspace_bytes(N, Cin, Cout), D3F_ERR_WORKSPACE,
               "unary_backward: workspace too small");
   if (dx != nullptr && N > 0) D3F_CUDA(cudaMemsetAsync(dx, 0, (size_t)N * Cin * sizeof(float), stream));
   if (dW != nullptr) D3F_CUDA(cudaMemsetAsync(dW, 0, (size_t)Cin * Cout * sizeof(float), stream));
   if (N == 0) return D3F_OK;
   Carver cv(workspace, workspace_bytes);
   float* WT = cv.take<float>((size_t)Cin * Cout);
-  float* WTp = cv.take<float>(tc_packed_floats(Cout, Cin));
+  float* WTp = cv.take<float>(d3f_packed_weight_floats(Cout, Cin));
   float* partial = cv.take<float>((size_t)wgrad_blocks(N) * Cin * Cout);
   int rc;
   if (dx != nullptr) {   // dx = dout @ W^T through the forward GEMM
@@ -446,7 +460,7 @@ int unary_backward(const float* x, const float* W, const float* dout, int N, int
     ep.row_map = nullptr;
     ep.m_dev = n_dev;
     if (tensor_cores && tc_gemm_supported(dout, Cout)) {
-      rc = tc_pack_weight(WT, Cout, Cin, WTp, stream);
+      rc = d3f_pack_weight(WT, Cout, Cin, WTp, stream);
       if (rc) return rc;
       rc = tc_gemm(dout, WTp, dx, N, Cin, Cout, ep, stream);
     } else {
@@ -463,5 +477,3 @@ int unary_backward(const float* x, const float* W, const float* dout, int N, int
   }
   return D3F_OK;
 }
-
-}  // namespace d3f

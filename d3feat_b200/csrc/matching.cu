@@ -198,28 +198,32 @@ match_finalize_kernel(const int* __restrict__ count, int B, int k, const int* __
 }
 
 }  // namespace
+}  // namespace d3f
 
-size_t match_descriptors_workspace_bytes(int k, int P) {
+using namespace d3f;
+
+extern "C" size_t d3f_match_descriptors_workspace_bytes(int k, int P) {
   if (k < 1 || P < 1 || (long long)P * k > INT32_MAX) return 0;
   return 2 * align_up(sizeof(unsigned long long) * (size_t)P * k, 256);
 }
 
-int match_descriptors(const float* desc, const int* count, int B, int k, int D, const int* pairs, int P, int* nn_st,
-                      float* sim_st, int* nn_ts, float* sim_ts, int* matches, int* n_matches, void* workspace,
-                      size_t workspace_bytes, cudaStream_t stream) {
+extern "C" int d3f_match_descriptors(const float* desc, const int* count, int B, int k, int D, const int* pairs, int P,
+                                     int* nn_st, float* sim_st, int* nn_ts, float* sim_ts, int* matches, int* n_matches,
+                                     void* workspace, size_t workspace_bytes, d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(B >= 1 && B <= kMaxBatch, D3F_ERR_INVALID, "match_descriptors: B=%d must be in [1,%d]", B, kMaxBatch);
   D3F_REQUIRE(k >= 1 && D >= 1 && P >= 1, D3F_ERR_INVALID, "match_descriptors: bad shape k=%d D=%d P=%d", k, D, P);
   D3F_REQUIRE((long long)P * k <= INT32_MAX, D3F_ERR_INVALID, "match_descriptors: P*k=%lld exceeds int32",
               (long long)P * k);
   D3F_REQUIRE(desc && count && pairs && nn_st && sim_st && nn_ts && sim_ts && matches && n_matches && workspace,
               D3F_ERR_INVALID, "match_descriptors: null pointer");
-  D3F_REQUIRE(workspace_bytes >= match_descriptors_workspace_bytes(k, P), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_match_descriptors_workspace_bytes(k, P), D3F_ERR_WORKSPACE,
               "match_descriptors: workspace too small");
   Carver cv(workspace, workspace_bytes);
   unsigned long long* row_key = cv.take<unsigned long long>((size_t)P * k);
   unsigned long long* col_key = cv.take<unsigned long long>((size_t)P * k);
   // key 0 is below every real key (score_ord is never 0): "no candidate yet"
-  D3F_CUDA(cudaMemsetAsync(workspace, 0, match_descriptors_workspace_bytes(k, P), stream));
+  D3F_CUDA(cudaMemsetAsync(workspace, 0, d3f_match_descriptors_workspace_bytes(k, P), stream));
   const int T = ceil_div(k, kTile);
   const long long tiles = (long long)P * T * T;
   const int blocks = (int)min(tiles, (long long)32 * kNumSMs);
@@ -231,5 +235,3 @@ int match_descriptors(const float* desc, const int* count, int B, int k, int D, 
   D3F_LAUNCH_CHECK("match_finalize_kernel");
   return D3F_OK;
 }
-
-}  // namespace d3f

@@ -78,16 +78,6 @@ static size_t carve_nb(Carver& cv, int Ns, int B, long long total_cells, NbWs& w
   return cv.off;
 }
 
-size_t radius_neighbors_workspace_bytes(int Ns, int B, float radius, const float* host_bbox) {
-  if (host_bbox == nullptr || !(radius > 0.f) || B < 1) return 0;
-  NbGrid g = make_grid(host_bbox, radius);
-  long long total = g.ncells * B;
-  if (total > kMaxGridCells || !radius_scan_complete(g)) return 0;
-  Carver cv(nullptr, ~(size_t)0);
-  NbWs w;
-  return carve_nb(cv, Ns, B, total, w) + 256;
-}
-
 int radius_neighbors_build(const float* supports, const int* s_batch_len, int B, int Ns, float radius,
                            const float* host_bbox, void* workspace, size_t workspace_bytes, cudaStream_t stream,
                            const int* ns_dev, const int* s_start_pre) {
@@ -102,7 +92,7 @@ int radius_neighbors_build(const float* supports, const int* s_batch_len, int B,
   D3F_REQUIRE(radius_scan_complete(g), D3F_ERR_INVALID,
               "radius_neighbors: grid %d x %d x %d has an axis longer than %d cells (of radius * 1.001)", g.nx, g.ny,
               g.nz, kMaxScanAxisCells);
-  D3F_REQUIRE(workspace_bytes >= radius_neighbors_workspace_bytes(Ns, B, radius, host_bbox), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_radius_neighbors_workspace_bytes(Ns, B, radius, host_bbox), D3F_ERR_WORKSPACE,
               "radius_neighbors: workspace too small");
   Carver cv(workspace, workspace_bytes);
   NbWs w;
@@ -121,23 +111,6 @@ int radius_neighbors_build(const float* supports, const int* s_batch_len, int B,
   cell_scatter_kernel<<<ceil_div(Ns, 256), 256, 0, stream>>>(supports, Ns, ns_dev, w.s_start, B, w.cell_id, w.cell_start,
                                                              w.cell_cnt, w.sorted_pts);
   D3F_LAUNCH_CHECK("cell_scatter_kernel");
-  return D3F_OK;
-}
-
-// Support indices in cell order (the payload of the sorted keys): a spatially coherent visiting order that
-// gather kernels can use for their queries when queries == supports.
-int radius_neighbors_order(const void* workspace, int Ns, int B, float radius, const float* host_bbox, int* out_order,
-                           cudaStream_t stream) {
-  D3F_REQUIRE(B >= 1 && radius > 0.f && host_bbox != nullptr, D3F_ERR_INVALID, "radius_neighbors_order: bad arguments");
-  if (Ns <= 0) return D3F_OK;
-  NbGrid g = make_grid(host_bbox, radius);
-  long long total = g.ncells * B;
-  D3F_REQUIRE(total <= kMaxGridCells, D3F_ERR_CAPACITY, "radius_neighbors: grid too large");
-  Carver cv(const_cast<void*>(workspace), ~(size_t)0);
-  NbWs w;
-  carve_nb(cv, Ns, B, total, w);
-  cell_order_kernel<<<ceil_div(Ns, 256), 256, 0, stream>>>(w.sorted_pts, Ns, out_order);
-  D3F_LAUNCH_CHECK("cell_order_kernel");
   return D3F_OK;
 }
 
@@ -663,14 +636,6 @@ static int query_common(bool fill, const float* queries, const int* q_batch_len,
   return D3F_OK;
 }
 
-int radius_neighbors_count(const float* queries, const int* q_batch_len, int Nq, int B, int Ns, float radius,
-                           const float* host_bbox, const void* workspace, int* counts, int* out_max,
-                           cudaStream_t stream) {
-  D3F_REQUIRE(counts != nullptr && out_max != nullptr, D3F_ERR_INVALID, "radius_neighbors_count: null output");
-  return query_common(false, queries, q_batch_len, Nq, B, Ns, radius, host_bbox, workspace, 0, 0, counts, out_max,
-                      nullptr, stream);
-}
-
 int radius_neighbors_fill(const float* queries, const int* q_batch_len, int Nq, int B, int Ns, float radius,
                           const float* host_bbox, const void* workspace, int cols, int pad_value, int* out_idx,
                           cudaStream_t stream, const int* nq_dev, const int* pad_dev, const int* q_start_pre) {
@@ -683,3 +648,68 @@ int radius_neighbors_fill(const float* queries, const int* q_batch_len, int Nq, 
 }
 
 }  // namespace d3f
+
+using namespace d3f;
+
+extern "C" size_t d3f_radius_neighbors_workspace_bytes(int Ns, int B, float radius, const float* host_bbox) {
+  if (host_bbox == nullptr || !(radius > 0.f) || B < 1) return 0;
+  NbGrid g = make_grid(host_bbox, radius);
+  long long total = g.ncells * B;
+  if (total > kMaxGridCells || !radius_scan_complete(g)) return 0;
+  Carver cv(nullptr, ~(size_t)0);
+  NbWs w;
+  return carve_nb(cv, Ns, B, total, w) + 256;
+}
+
+extern "C" int d3f_radius_neighbors_build(const float* supports, const int* s_batch_len, int B, int Ns, float radius,
+                                          const float* host_bbox, void* workspace, size_t workspace_bytes,
+                                          d3f_stream_t stream) {
+  D3F_REQUIRE((supports != nullptr || Ns == 0) && s_batch_len != nullptr && workspace != nullptr, D3F_ERR_INVALID,
+              "d3f_radius_neighbors_build: null pointer");
+  return radius_neighbors_build(supports, s_batch_len, B, Ns, radius, host_bbox, workspace, workspace_bytes,
+                                (cudaStream_t)stream);
+}
+
+extern "C" int d3f_radius_neighbors_count(const float* queries, const int* q_batch_len, int Nq, const float* supports,
+                                          const int* s_batch_len, int B, int Ns, float radius, const float* host_bbox,
+                                          const void* workspace, int* counts, int* out_max, d3f_stream_t stream) {
+  (void)supports;
+  (void)s_batch_len;
+  D3F_REQUIRE((queries != nullptr || Nq == 0) && q_batch_len != nullptr && workspace != nullptr, D3F_ERR_INVALID,
+              "d3f_radius_neighbors_count: null pointer");
+  D3F_REQUIRE(counts != nullptr && out_max != nullptr, D3F_ERR_INVALID, "radius_neighbors_count: null output");
+  return query_common(false, queries, q_batch_len, Nq, B, Ns, radius, host_bbox, workspace, 0, 0, counts, out_max,
+                      nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int d3f_radius_neighbors_fill(const float* queries, const int* q_batch_len, int Nq, const float* supports,
+                                         const int* s_batch_len, int B, int Ns, float radius, const float* host_bbox,
+                                         const void* workspace, int cols, int pad_value, int* out_idx,
+                                         d3f_stream_t stream) {
+  (void)supports;
+  (void)s_batch_len;
+  D3F_REQUIRE((queries != nullptr || Nq == 0) && q_batch_len != nullptr && workspace != nullptr, D3F_ERR_INVALID,
+              "d3f_radius_neighbors_fill: null pointer");
+  return radius_neighbors_fill(queries, q_batch_len, Nq, B, Ns, radius, host_bbox, workspace, cols, pad_value, out_idx,
+                               (cudaStream_t)stream);
+}
+
+// Support indices in cell order (the payload of the sorted keys): a spatially coherent visiting order that
+// gather kernels can use for their queries when queries == supports.
+extern "C" int d3f_radius_neighbors_order(const void* workspace, int Ns, int B, float radius, const float* host_bbox,
+                                          int* out_order, d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  D3F_REQUIRE(workspace != nullptr && (out_order != nullptr || Ns == 0), D3F_ERR_INVALID,
+              "d3f_radius_neighbors_order: null pointer");
+  D3F_REQUIRE(B >= 1 && radius > 0.f && host_bbox != nullptr, D3F_ERR_INVALID, "radius_neighbors_order: bad arguments");
+  if (Ns <= 0) return D3F_OK;
+  NbGrid g = make_grid(host_bbox, radius);
+  long long total = g.ncells * B;
+  D3F_REQUIRE(total <= kMaxGridCells, D3F_ERR_CAPACITY, "radius_neighbors: grid too large");
+  Carver cv(const_cast<void*>(workspace), ~(size_t)0);
+  NbWs w;
+  carve_nb(cv, Ns, B, total, w);
+  cell_order_kernel<<<ceil_div(Ns, 256), 256, 0, stream>>>(w.sorted_pts, Ns, out_order);
+  D3F_LAUNCH_CHECK("cell_order_kernel");
+  return D3F_OK;
+}

@@ -95,8 +95,17 @@ ind_max_pool_fix_kernel(const int* __restrict__ inds, int N1cap, int N2cap, cons
   }
 }
 
-int ind_max_pool(const float* x, const int* inds, int N1, int N2, int H, int C, float* out, void* workspace,
-                 size_t workspace_bytes, cudaStream_t stream, const int* n1_dev, const int* n2_dev) {
+}  // namespace d3f
+
+using namespace d3f;
+
+extern "C" size_t d3f_ind_max_pool_workspace_bytes(int C) { return sizeof(unsigned) * ((size_t)(C > 0 ? C : 1) + 1); }
+
+extern "C" int d3f_ind_max_pool(const float* x, const int* inds, int N1, int N2, int H, int C, float* out,
+                                void* workspace, size_t workspace_bytes, d3f_stream_t stream_, const int* n1_dev,
+                                const int* n2_dev) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  D3F_REQUIRE(N2 == 0 || (x && inds && out && workspace), D3F_ERR_INVALID, "d3f_ind_max_pool: null pointer");
   D3F_REQUIRE(N1 >= 1 && N2 >= 0 && H >= 0 && C >= 1, D3F_ERR_INVALID, "ind_max_pool: bad shape N1=%d N2=%d H=%d C=%d",
               N1, N2, H, C);
   D3F_REQUIRE(workspace_bytes >= sizeof(unsigned) * ((size_t)C + 1), D3F_ERR_WORKSPACE,
@@ -120,6 +129,8 @@ int ind_max_pool(const float* x, const int* inds, int N1, int N2, int H, int C, 
   return D3F_OK;
 }
 
+namespace d3f {
+
 __global__ void __launch_bounds__(256)
 closest_pool_kernel(const float* __restrict__ x, const int* __restrict__ inds, int N1cap, int N2cap,
                     const int* __restrict__ n1_dev, const int* __restrict__ n2_dev, int ld, int C,
@@ -132,14 +143,20 @@ closest_pool_kernel(const float* __restrict__ x, const int* __restrict__ inds, i
   for (int c = lane; c < C; c += 32) out[(size_t)warp * C + c] = shadow ? 0.f : x[(size_t)id * C + c];
 }
 
-int closest_pool(const float* x, const int* inds, int N1, int N2, int ld_inds, int C, float* out, cudaStream_t stream,
-                 const int* n1_dev, const int* n2_dev) {
+}  // namespace d3f
+
+extern "C" int d3f_closest_pool(const float* x, const int* inds, int N1, int N2, int ld_inds, int C, float* out,
+                                d3f_stream_t stream_, const int* n1_dev, const int* n2_dev) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  D3F_REQUIRE(N2 == 0 || (x && inds && out), D3F_ERR_INVALID, "d3f_closest_pool: null pointer");
   D3F_REQUIRE(N1 >= 0 && N2 >= 0 && ld_inds >= 1 && C >= 1, D3F_ERR_INVALID, "closest_pool: bad shape");
   if (N2 == 0) return D3F_OK;
   closest_pool_kernel<<<ceil_div(N2 * 32, 256), 256, 0, stream>>>(x, inds, N1, N2, n1_dev, n2_dev, ld_inds, C, out);
   D3F_LAUNCH_CHECK("closest_pool_kernel");
   return D3F_OK;
 }
+
+namespace d3f {
 
 __global__ void __launch_bounds__(256) l2_normalize_kernel(const float* __restrict__ x, int Ncap,
                                                            const int* __restrict__ n_dev, int C, float eps,
@@ -161,13 +178,20 @@ __global__ void __launch_bounds__(256) l2_normalize_kernel(const float* __restri
   for (int c = lane; c < C; c += 32) out[(size_t)warp * C + c] = x[(size_t)warp * C + c] * inv;
 }
 
-int l2_normalize(const float* x, int N, int C, float eps, float* out, cudaStream_t stream, const int* n_dev) {
+}  // namespace d3f
+
+extern "C" int d3f_l2_normalize(const float* x, int N, int C, float eps, float* out, d3f_stream_t stream_,
+                                const int* n_dev) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  D3F_REQUIRE(N == 0 || (x && out), D3F_ERR_INVALID, "d3f_l2_normalize: null pointer");
   D3F_REQUIRE(N >= 0 && C >= 1, D3F_ERR_INVALID, "l2_normalize: bad shape");
   if (N == 0) return D3F_OK;
   l2_normalize_kernel<<<ceil_div(N * 32, 256), 256, 0, stream>>>(x, N, n_dev, C, eps, out);
   D3F_LAUNCH_CHECK("l2_normalize_kernel");
   return D3F_OK;
 }
+
+namespace d3f {
 
 // ---------------------------------------------------------------------------------------------------
 // Detection score of D3Feat (models/D3Feat.py:67-115), generalised from the reference's hard-coded pair of clouds to
@@ -238,15 +262,20 @@ detection_score_kernel(const float* __restrict__ x, const int* __restrict__ nb, 
   if (lane == 0) score[warp] = best;
 }
 
-size_t detection_scores_workspace_bytes(int N, int B) {
+}  // namespace d3f
+
+extern "C" size_t d3f_detection_scores_workspace_bytes(int N, int B) {
   return align_up(sizeof(int) * (size_t)(B + 1), 256) + align_up(sizeof(unsigned) * (size_t)B, 256) + align_up((size_t)N + 1, 256);
 }
 
-int detection_scores(const float* feats, const int* neighbors, const int* lengths, int B, int N, int H, int D,
-                     float* out_scores, void* workspace, size_t workspace_bytes, cudaStream_t stream,
-                     const int* n_dev) {
+extern "C" int d3f_detection_scores(const float* feats, const int* neighbors, const int* lengths, int B, int N, int H,
+                                    int D, float* out_scores, void* workspace, size_t workspace_bytes,
+                                    d3f_stream_t stream_, const int* n_dev) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  D3F_REQUIRE(N == 0 || (feats && (neighbors || H == 0) && lengths && out_scores && workspace), D3F_ERR_INVALID,
+              "d3f_detection_scores: null pointer");
   D3F_REQUIRE(B >= 1 && B <= kMaxBatch && N >= 0 && H >= 0 && D >= 1, D3F_ERR_INVALID, "detection_scores: bad shape");
-  D3F_REQUIRE(workspace_bytes >= detection_scores_workspace_bytes(N, B), D3F_ERR_WORKSPACE, "detection_scores: workspace too small");
+  D3F_REQUIRE(workspace_bytes >= d3f_detection_scores_workspace_bytes(N, B), D3F_ERR_WORKSPACE, "detection_scores: workspace too small");
   if (N == 0) return D3F_OK;
   Carver cv(workspace, workspace_bytes);
   int* start = cv.take<int>(B + 1);
@@ -261,6 +290,8 @@ int detection_scores(const float* feats, const int* neighbors, const int* length
   D3F_LAUNCH_CHECK("detection_score_kernel");
   return D3F_OK;
 }
+
+namespace d3f {
 
 __global__ void __launch_bounds__(256)
 affine_leaky_kernel(const float* __restrict__ x, long long total_cap, const int* __restrict__ n_dev, int C,
@@ -277,8 +308,13 @@ affine_leaky_kernel(const float* __restrict__ x, long long total_cap, const int*
   }
 }
 
-int affine_leaky(const float* x, int N, int C, const float* scale, const float* shift, const float* residual,
-                 float alpha, float* out, cudaStream_t stream, const int* n_dev) {
+}  // namespace d3f
+
+extern "C" int d3f_affine_leaky(const float* x, int N, int C, const float* scale, const float* shift,
+                                const float* residual, float alpha, float* out, d3f_stream_t stream_,
+                                const int* n_dev) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  D3F_REQUIRE(N == 0 || (x && out), D3F_ERR_INVALID, "d3f_affine_leaky: null pointer");
   D3F_REQUIRE(N >= 0 && C >= 1 && (scale == nullptr) == (shift == nullptr), D3F_ERR_INVALID, "affine_leaky: bad arguments");
   long long total = (long long)N * C;
   if (total == 0) return D3F_OK;
@@ -287,5 +323,3 @@ int affine_leaky(const float* x, int N, int C, const float* scale, const float* 
   D3F_LAUNCH_CHECK("affine_leaky_kernel");
   return D3F_OK;
 }
-
-}  // namespace d3f

@@ -29,13 +29,22 @@ inline bool same_radius(float a, float b) { return fabsf(a - b) <= 1e-6f * fmaxf
 
 }  // namespace
 
+__global__ void set_count_kernel(int* __restrict__ dst, int value, const int* __restrict__ src) {
+  *dst = src ? *src : value;
+}
+
+}  // namespace d3f
+
+using namespace d3f;
+
 // Workspace: one subsampling workspace (level-0 sized) + one grid workspace per distinct (level, radius) pair,
 // sized with the per-level row capacity.
-size_t pyramid_workspace_bytes(int B, const d3f_pyramid_spec* spec, const int* capacity, const float* host_bbox) {
+extern "C" size_t d3f_pyramid_workspace_bytes(int B, const d3f_pyramid_spec* spec, const int* capacity,
+                                              const float* host_bbox) {
   if (spec == nullptr || capacity == nullptr || host_bbox == nullptr) return 0;
   int L = spec->n_levels;
   if (L < 1 || L > D3F_MAX_LEVELS) return 0;
-  size_t total = align_up(grid_subsample_workspace_bytes(capacity[0], B) + 512, 256);
+  size_t total = align_up(d3f_grid_subsample_workspace_bytes(capacity[0], B) + 512, 256);
   total += align_up(sizeof(int) * (size_t)D3F_MAX_LEVELS * (B + 1), 256);   // exclusive scans of every level's lengths
   for (int l = 0; l < L; ++l) {
     float radii[3] = {spec->conv_radius[l], spec->sub_dl[l] > 0.f ? spec->pool_radius[l] : -1.f,
@@ -45,16 +54,12 @@ size_t pyramid_workspace_bytes(int B, const d3f_pyramid_spec* spec, const int* c
       bool dup = false;
       for (int b = 0; b < a; ++b) dup = dup || (radii[b] > 0.f && same_radius(radii[a], radii[b]));
       if (dup) continue;
-      size_t nb = radius_neighbors_workspace_bytes(capacity[l], B, radii[a], host_bbox);
+      size_t nb = d3f_radius_neighbors_workspace_bytes(capacity[l], B, radii[a], host_bbox);
       if (nb == 0) return 0;
       total += align_up(nb, 256);
     }
   }
   return total + 1024;
-}
-
-__global__ void set_count_kernel(int* __restrict__ dst, int value, const int* __restrict__ src) {
-  *dst = src ? *src : value;
 }
 
 // Two ways to run it:
@@ -66,11 +71,16 @@ __global__ void set_count_kernel(int* __restrict__ dst, int value, const int* __
 //    bbox) are OR-ed into *d_status. The launch sequence then depends on nothing but (B, capacity, spec, bbox): it
 //    can be captured once as a CUDA graph and replayed for every batch of the bucket.
 // d_counts[0] is N0, or *n0_dev when the caller keeps the level-0 count on the device (graph replay: N0 = capacity[0]).
-int pyramid_build(const float* points, const int* lengths, int B, int N0, const d3f_pyramid_spec* spec,
-                  const float* host_bbox, float* const* out_points, int* const* out_lengths,
-                  int* const* out_neighbors, int* const* out_pools, int* const* out_upsamples, const int* capacity,
-                  int* out_level_sizes, void* workspace, size_t workspace_bytes, cudaStream_t stream, int* d_counts,
-                  int* d_status, const int* n0_dev) {
+extern "C" int d3f_pyramid_build(const float* points, const int* lengths, int B, int N0, const d3f_pyramid_spec* spec,
+                                 const float* host_bbox, float* const* out_points, int* const* out_lengths,
+                                 int* const* out_neighbors, int* const* out_pools, int* const* out_upsamples,
+                                 const int* capacity, int* out_level_sizes, void* workspace, size_t workspace_bytes,
+                                 d3f_stream_t stream_, int* d_counts, int* d_status, const int* n0_dev) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  D3F_REQUIRE((points != nullptr || N0 == 0) && lengths != nullptr && out_points && out_lengths && out_neighbors &&
+                  out_pools && out_upsamples && workspace,
+              D3F_ERR_INVALID, "d3f_pyramid_build: null pointer");
+  D3F_REQUIRE(B >= 1 && B <= kMaxBatch, D3F_ERR_INVALID, "d3f_pyramid_build: B=%d", B);
   D3F_REQUIRE(spec != nullptr && capacity != nullptr && host_bbox != nullptr, D3F_ERR_INVALID,
               "pyramid_build: null argument");
   const bool exact = out_level_sizes != nullptr;
@@ -79,14 +89,14 @@ int pyramid_build(const float* points, const int* lengths, int B, int N0, const 
   const int L = spec->n_levels;
   D3F_REQUIRE(L >= 1 && L <= D3F_MAX_LEVELS, D3F_ERR_INVALID, "pyramid_build: n_levels=%d", L);
   D3F_REQUIRE(N0 >= 0 && N0 <= capacity[0], D3F_ERR_CAPACITY, "pyramid_build: N0=%d exceeds capacity %d", N0, capacity[0]);
-  D3F_REQUIRE(workspace_bytes >= pyramid_workspace_bytes(B, spec, capacity, host_bbox) &&
-                  pyramid_workspace_bytes(B, spec, capacity, host_bbox) > 0,
+  D3F_REQUIRE(workspace_bytes >= d3f_pyramid_workspace_bytes(B, spec, capacity, host_bbox) &&
+                  d3f_pyramid_workspace_bytes(B, spec, capacity, host_bbox) > 0,
               D3F_ERR_WORKSPACE, "pyramid_build: workspace too small (or grid too large)");
 
   char* base = (char*)workspace;
   size_t off = 0;
   void* sub_ws = base;
-  size_t sub_bytes = align_up(grid_subsample_workspace_bytes(capacity[0], B) + 512, 256);
+  size_t sub_bytes = align_up(d3f_grid_subsample_workspace_bytes(capacity[0], B) + 512, 256);
   off += sub_bytes;
   // start[l][b] = first row of cloud b at level l: scanned ONCE per level (every grid build, search and subsampling
   // of that level used to launch its own scan: 22 launches per step instead of 5)
@@ -119,7 +129,7 @@ int pyramid_build(const float* points, const int* lengths, int B, int N0, const 
     GridSlot& g = slots[n_slots];
     g.level = l;
     g.radius = radius;
-    g.bytes = align_up(radius_neighbors_workspace_bytes(capacity[l], B, radius, host_bbox), 256);
+    g.bytes = align_up(d3f_radius_neighbors_workspace_bytes(capacity[l], B, radius, host_bbox), 256);
     g.ws = base + off;
     off += g.bytes;
     D3F_REQUIRE(off <= workspace_bytes, D3F_ERR_WORKSPACE, "pyramid_build: workspace exhausted");
@@ -182,5 +192,3 @@ int pyramid_build(const float* points, const int* lengths, int B, int N0, const 
   }
   return D3F_OK;
 }
-
-}  // namespace d3f

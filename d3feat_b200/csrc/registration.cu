@@ -441,18 +441,23 @@ bool sizes_ok(int L, int P, int T, int V) {
 }
 
 }  // namespace
+}  // namespace d3f
 
-size_t register_pairs_workspace_bytes(int L, int P, int max_iterations, int max_validation) {
+using namespace d3f;
+
+extern "C" size_t d3f_register_pairs_workspace_bytes(int L, int P, int max_iterations, int max_validation) {
   if (!sizes_ok(L, P, max_iterations, max_validation)) return 0;
   const size_t P_ = (size_t)P, V = (size_t)max_validation;
   return 2 * align_up(sizeof(int) * P_, 256) + align_up(sizeof(unsigned) * P_ * ceil_div(max_iterations, 32), 256) +
          2 * align_up(sizeof(int) * P_ * V, 256) + align_up(sizeof(double) * P_ * V, 256);
 }
 
-int register_pairs(const float* points, const int* count, int B, int k, const int* corr, const int* n_corr, int L,
-                   const int* pairs, int P, int ransac_n, int max_iterations, int max_validation, double distance,
-                   double edge_ratio, unsigned long long seed, double* pose, int* n_inliers, int* hypothesis,
-                   int* n_validated, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+extern "C" int d3f_register_pairs(const float* points, const int* count, int B, int k, const int* corr,
+                                  const int* n_corr, int L, const int* pairs, int P, int ransac_n, int max_iterations,
+                                  int max_validation, double distance, double edge_ratio, unsigned long long seed,
+                                  double* pose, int* n_inliers, int* hypothesis, int* n_validated, void* workspace,
+                                  size_t workspace_bytes, d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(B >= 1 && B <= kMaxBatch, D3F_ERR_INVALID, "register_pairs: B=%d must be in [1,%d]", B, kMaxBatch);
   D3F_REQUIRE(k >= 1 && L >= 1 && P >= 1, D3F_ERR_INVALID, "register_pairs: bad shape k=%d L=%d P=%d", k, L, P);
   D3F_REQUIRE(ransac_n >= 3 && ransac_n <= 8, D3F_ERR_INVALID, "register_pairs: ransac_n=%d must be in [3,8]",
@@ -470,7 +475,7 @@ int register_pairs(const float* points, const int* count, int B, int k, const in
   D3F_REQUIRE(points && count && corr && n_corr && pairs && pose && n_inliers && hypothesis && n_validated &&
                   workspace,
               D3F_ERR_INVALID, "register_pairs: null pointer");
-  const size_t need = register_pairs_workspace_bytes(L, P, max_iterations, max_validation);
+  const size_t need = d3f_register_pairs_workspace_bytes(L, P, max_iterations, max_validation);
   D3F_REQUIRE(workspace_bytes >= need, D3F_ERR_WORKSPACE, "register_pairs: workspace too small (%zu < %zu bytes)",
               workspace_bytes, need);
   const Work w = carve(workspace, workspace_bytes, P, max_iterations, max_validation);
@@ -492,5 +497,3 @@ int register_pairs(const float* points, const int* count, int B, int k, const in
                            hypothesis, n_validated, w, stream);
   }
 }
-
-}  // namespace d3f

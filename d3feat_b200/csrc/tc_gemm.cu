@@ -52,12 +52,18 @@ __global__ void __launch_bounds__(256) pack_weight_kernel(const float* __restric
   }
 }
 
-int tc_padded_k(int K) { return (K + kTcBK - 1) / kTcBK * kTcBK; }
-int tc_block_n(int N) { return N > 64 ? 128 : (N > 32 ? 64 : 32); }
-int tc_padded_n(int N) { int bn = tc_block_n(N); return (N + bn - 1) / bn * bn; }
-size_t tc_packed_floats(int K, int N) { return 2 * (size_t)tc_padded_k(K) * tc_padded_n(N); }
+static int tc_padded_k(int K) { return (K + kTcBK - 1) / kTcBK * kTcBK; }
+static int tc_block_n(int N) { return N > 64 ? 128 : (N > 32 ? 64 : 32); }
+static int tc_padded_n(int N) { int bn = tc_block_n(N); return (N + bn - 1) / bn * bn; }
 
-int tc_pack_weight(const float* W, int K, int N, float* packed, cudaStream_t stream) {
+}  // namespace d3f
+
+using namespace d3f;
+
+extern "C" size_t d3f_packed_weight_floats(int K, int N) { return 2 * (size_t)tc_padded_k(K) * tc_padded_n(N); }
+
+extern "C" int d3f_pack_weight(const float* W, int K, int N, float* packed, d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(K >= 1 && N >= 1 && W && packed, D3F_ERR_INVALID, "pack_weight: bad arguments");
   int Kpad = tc_padded_k(K), Npad = tc_padded_n(N);
   long long total = (long long)Npad * Kpad;
@@ -66,6 +72,8 @@ int tc_pack_weight(const float* W, int K, int N, float* packed, cudaStream_t str
   D3F_LAUNCH_CHECK("pack_weight_kernel");
   return D3F_OK;
 }
+
+namespace d3f {
 
 // ---------------------------------------------------------------------------------------------------
 // Accumulation. Each k-chunk (12 wgmmas) is summed into a fresh register fragment that the consumer adds to the running
@@ -424,12 +432,12 @@ bool tc_gemm_supported(const float* A, int K) {
   return (K % 4 == 0) && ((reinterpret_cast<uintptr_t>(A) & 15) == 0);
 }
 
-// A[M,K] fp32 row-major, Bp = packed weight (tc_pack_weight), C[M,N]
+// A[M,K] fp32 row-major, Bp = packed weight (d3f_pack_weight), C[M,N]
 // split-K plan for GEMMs that cannot fill the GPU with output tiles: returns the number of K splits (1 = none)
 // Deterministic split-K plan for GEMMs whose output tiles cannot fill the GPU. The k-loop of a CTA is latency bound
 // (about a microsecond per k-chunk), so the cost of a plan is (waves of CTAs) x (k-chunks per CTA) plus the extra
 // pass of the reduction; the cheapest of s = 1..8 wins. Returns the number of K splits (1 = none).
-int tc_gemm_splits(int M, int N, int K) {
+static int tc_gemm_splits(int M, int N, int K) {
   const int bn = tc_block_n(N);
   const long long ctas = (long long)ceil_div(M, kTcBM) * (tc_padded_n(N) / bn);
   const int nk = tc_padded_k(K) / kTcBK;
@@ -486,3 +494,23 @@ int tc_gemm(const float* A, const float* Bp, float* C, int M, int N, int K, cons
 }
 
 }  // namespace d3f
+
+extern "C" int d3f_unary_pair_forward(const float* x1, int Cin1, const float* x2, int Cin2, const float* W_packed,
+                                      int N, int Cout, const float* shift, float leaky_alpha, float* out,
+                                      d3f_stream_t stream, const int* n_dev) {
+  D3F_REQUIRE(N >= 0 && Cin1 >= 1 && Cin2 >= 1 && Cout >= 1, D3F_ERR_INVALID,
+              "d3f_unary_pair_forward: bad shape N=%d Cin=%d+%d Cout=%d", N, Cin1, Cin2, Cout);
+  D3F_REQUIRE(N == 0 || (x1 && x2 && W_packed && out), D3F_ERR_INVALID, "d3f_unary_pair_forward: null pointer");
+  D3F_REQUIRE(Cin1 % 32 == 0 && Cin2 % 4 == 0, D3F_ERR_INVALID,
+              "d3f_unary_pair_forward: Cin1 must be a multiple of 32 and Cin2 of 4 (got %d, %d)", Cin1, Cin2);
+  Epilogue ep;
+  ep.rowscale = nullptr;
+  ep.bn_scale = nullptr;
+  ep.bn_shift = nullptr;
+  ep.bias = shift;
+  ep.residual = nullptr;
+  ep.leaky_alpha = leaky_alpha;
+  ep.row_map = nullptr;
+  ep.m_dev = n_dev;
+  return tc_gemm(x1, W_packed, out, N, Cout, Cin1 + Cin2, ep, (cudaStream_t)stream, nullptr, x2, Cin1);
+}

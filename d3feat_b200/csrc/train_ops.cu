@@ -173,15 +173,21 @@ __global__ void __launch_bounds__(256) bn_dx_kernel(const float* __restrict__ x,
   }
 }
 
-size_t batch_norm_train_workspace_bytes(int N, int C) {
+}  // namespace d3f
+
+using namespace d3f;
+
+extern "C" size_t d3f_batch_norm_train_workspace_bytes(int N, int C) {
   if (N < 0 || C < 1) return 0;
   const size_t nb = (size_t)row_blocks(N) * C;
   return 2 * align_up(nb * sizeof(double), 256) + 6 * align_up((size_t)C * sizeof(float), 256) + 1024;
 }
 
-int batch_norm_train_forward(const float* x, int N, int C, const float* gamma, const float* beta, float* moving_mean,
-                             float* moving_var, float decay, float eps, const float* residual, float alpha, float* out,
-                             float* mean, float* invstd, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+extern "C" int d3f_batch_norm_train_forward(const float* x, int N, int C, const float* gamma, const float* beta,
+                                            float* moving_mean, float* moving_var, float decay, float eps,
+                                            const float* residual, float alpha, float* out, float* mean, float* invstd,
+                                            void* workspace, size_t workspace_bytes, d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(N >= 0 && C >= 1 && (long long)N * C < (1ll << 31), D3F_ERR_INVALID,
               "batch_norm_train_forward: bad shape N=%d C=%d", N, C);
   D3F_REQUIRE(decay >= 0.f && decay <= 1.f && eps > 0.f, D3F_ERR_INVALID,
@@ -189,7 +195,7 @@ int batch_norm_train_forward(const float* x, int N, int C, const float* gamma, c
               (double)eps);
   D3F_REQUIRE(beta != nullptr && (gamma == nullptr || (moving_mean && moving_var && mean && invstd)),
               D3F_ERR_INVALID, "batch_norm_train_forward: null pointer");
-  D3F_REQUIRE(workspace_bytes >= batch_norm_train_workspace_bytes(N, C), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_batch_norm_train_workspace_bytes(N, C), D3F_ERR_WORKSPACE,
               "batch_norm_train_forward: workspace too small");
   if (N == 0) return D3F_OK;   // no batch statistics: the moving statistics stay as they are
   D3F_REQUIRE(x && out && workspace, D3F_ERR_INVALID, "batch_norm_train_forward: null pointer");
@@ -216,18 +222,19 @@ int batch_norm_train_forward(const float* x, int N, int C, const float* gamma, c
     offset_affine_kernel<<<cb, 256, 0, stream>>>(beta, C, scale, shift);
     D3F_LAUNCH_CHECK("offset_affine_kernel");
   }
-  return affine_leaky(x, N, C, scale, shift, residual, alpha, out, stream);
+  return d3f_affine_leaky(x, N, C, scale, shift, residual, alpha, out, stream, nullptr);
 }
 
-int batch_norm_train_backward(const float* x, const float* out, const float* dout, int N, int C, const float* gamma,
-                              const float* mean, const float* invstd, float alpha, float* dx, float* dresidual,
-                              float* dgamma, float* dbeta, void* workspace, size_t workspace_bytes,
-                              cudaStream_t stream) {
+extern "C" int d3f_batch_norm_train_backward(const float* x, const float* out, const float* dout, int N, int C,
+                                             const float* gamma, const float* mean, const float* invstd, float alpha,
+                                             float* dx, float* dresidual, float* dgamma, float* dbeta, void* workspace,
+                                             size_t workspace_bytes, d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(N >= 0 && C >= 1 && (long long)N * C < (1ll << 31), D3F_ERR_INVALID,
               "batch_norm_train_backward: bad shape N=%d C=%d", N, C);
   D3F_REQUIRE(gamma != nullptr || dgamma == nullptr, D3F_ERR_INVALID,
               "batch_norm_train_backward: dgamma without gamma (use_batch_norm = False has no gamma)");
-  D3F_REQUIRE(workspace_bytes >= batch_norm_train_workspace_bytes(N, C), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_batch_norm_train_workspace_bytes(N, C), D3F_ERR_WORKSPACE,
               "batch_norm_train_backward: workspace too small");
   if (dgamma) D3F_CUDA(cudaMemsetAsync(dgamma, 0, (size_t)C * sizeof(float), stream));
   if (dbeta) D3F_CUDA(cudaMemsetAsync(dbeta, 0, (size_t)C * sizeof(float), stream));
@@ -253,6 +260,8 @@ int batch_norm_train_backward(const float* x, const float* out, const float* dou
   }
   return D3F_OK;
 }
+
+namespace d3f {
 
 // ---- ind_max_pool backward ----------------------------------------------------------------------------------------
 // column minimum (ordered uint, preset 0xFFFFFFFF) or, with cmin given, the number of rows equal to it
@@ -382,22 +391,26 @@ static MaxPoolBwd carve_maxpool(Carver& cv, int N1, int N2, int H, int C) {
   return w;
 }
 
-size_t ind_max_pool_backward_workspace_bytes(int N1, int N2, int H, int C) {
+}  // namespace d3f
+
+extern "C" size_t d3f_ind_max_pool_backward_workspace_bytes(int N1, int N2, int H, int C) {
   if (N1 < 1 || N2 < 0 || H < 0 || C < 1 || (long long)N2 * H >= (1ll << 31)) return 0;
   Carver cv(nullptr, 0);
   carve_maxpool(cv, N1, N2, H, C);
   return cv.off + 1024;
 }
 
-int ind_max_pool_backward(const float* x, const int* inds, const float* out, const float* dout, int N1, int N2, int H,
-                          int C, float* dx, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+extern "C" int d3f_ind_max_pool_backward(const float* x, const int* inds, const float* out, const float* dout, int N1,
+                                         int N2, int H, int C, float* dx, void* workspace, size_t workspace_bytes,
+                                         d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(N1 >= 1 && N2 >= 0 && H >= 0 && C >= 1, D3F_ERR_INVALID,
               "ind_max_pool_backward: bad shape N1=%d N2=%d H=%d C=%d", N1, N2, H, C);
   D3F_REQUIRE((long long)N2 * max(H, C) < (1ll << 31) && (long long)N1 * C < (1ll << 31), D3F_ERR_INVALID,
               "ind_max_pool_backward: N2*H, N2*C or N1*C beyond int32");
   D3F_REQUIRE(x && dx && (N2 == 0 || (inds && out && dout && workspace)), D3F_ERR_INVALID,
               "ind_max_pool_backward: null pointer");
-  D3F_REQUIRE(workspace_bytes >= ind_max_pool_backward_workspace_bytes(N1, N2, H, C), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_ind_max_pool_backward_workspace_bytes(N1, N2, H, C), D3F_ERR_WORKSPACE,
               "ind_max_pool_backward: workspace too small");
   if (N2 == 0 || H == 0) {   // nothing was pooled (H = 0: every pooled row is the column minimum of no entry)
     D3F_CUDA(cudaMemsetAsync(dx, 0, (size_t)N1 * C * sizeof(float), stream));
@@ -431,6 +444,8 @@ int ind_max_pool_backward(const float* x, const int* inds, const float* out, con
   return D3F_OK;
 }
 
+namespace d3f {
+
 // ---- gather backward (closest_pool, tf.gather) --------------------------------------------------------------------
 // dx[s,c] = sum of dout[q,c] over the q with inds[q] == s, ascending q, float64, one rounding
 __global__ void __launch_bounds__(256) gather_rows_grad_kernel(const float* __restrict__ dout,
@@ -447,21 +462,24 @@ __global__ void __launch_bounds__(256) gather_rows_grad_kernel(const float* __re
   }
 }
 
-size_t gather_rows_backward_workspace_bytes(int N1, int N2) {
+}  // namespace d3f
+
+extern "C" size_t d3f_gather_rows_backward_workspace_bytes(int N1, int N2) {
   if (N1 < 0 || N2 < 0) return 0;
   Carver cv(nullptr, 0);
   carve_csr(cv, N2, N1);
   return cv.off + 1024;
 }
 
-int gather_rows_backward(const int* inds, const float* dout, int N1, int N2, int C, float* dx, void* workspace,
-                         size_t workspace_bytes, cudaStream_t stream) {
+extern "C" int d3f_gather_rows_backward(const int* inds, const float* dout, int N1, int N2, int C, float* dx,
+                                        void* workspace, size_t workspace_bytes, d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(N1 >= 0 && N2 >= 0 && C >= 1 && (long long)max(N1, N2) * C < (1ll << 31), D3F_ERR_INVALID,
               "gather_rows_backward: bad shape N1=%d N2=%d C=%d", N1, N2, C);
   D3F_REQUIRE(N1 == 0 || dx, D3F_ERR_INVALID, "gather_rows_backward: null pointer");
   D3F_REQUIRE(N1 == 0 || N2 == 0 || (inds && dout && workspace), D3F_ERR_INVALID,
               "gather_rows_backward: null pointer");
-  D3F_REQUIRE(workspace_bytes >= gather_rows_backward_workspace_bytes(N1, N2), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_gather_rows_backward_workspace_bytes(N1, N2), D3F_ERR_WORKSPACE,
               "gather_rows_backward: workspace too small");
   if (N1 == 0) return D3F_OK;
   if (N2 == 0) {
@@ -478,6 +496,8 @@ int gather_rows_backward(const int* inds, const float* dout, int N1, int N2, int
   D3F_LAUNCH_CHECK("gather_rows_grad_kernel");
   return D3F_OK;
 }
+
+namespace d3f {
 
 // ---- l2_normalize backward ------------------------------------------------------------------------------------------
 // one warp per row; sum x^2 and the reciprocal norm exactly as the forward computes them. sum x^2 >= eps (Maximum's
@@ -512,7 +532,11 @@ __global__ void __launch_bounds__(256) l2_normalize_grad_kernel(const float* __r
   }
 }
 
-int l2_normalize_backward(const float* x, const float* dout, int N, int C, float eps, float* dx, cudaStream_t stream) {
+}  // namespace d3f
+
+extern "C" int d3f_l2_normalize_backward(const float* x, const float* dout, int N, int C, float eps, float* dx,
+                                         d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(N >= 0 && C >= 1 && eps > 0.f, D3F_ERR_INVALID, "l2_normalize_backward: bad arguments N=%d C=%d eps=%g", N,
               C, (double)eps);
   if (N == 0) return D3F_OK;
@@ -521,6 +545,8 @@ int l2_normalize_backward(const float* x, const float* dout, int N, int C, float
   D3F_LAUNCH_CHECK("l2_normalize_grad_kernel");
   return D3F_OK;
 }
+
+namespace d3f {
 
 // ---- detection_scores backward ------------------------------------------------------------------------------------
 // Forward (pool.cu), row i of cloud b, inv = 1/(M_b + 1e-6) with M_b the cloud's maximum, cnt = neighbours with a
@@ -739,21 +765,24 @@ static DetBwd carve_det(Carver& cv, int N, int H, int B, int D) {
   return w;
 }
 
-size_t detection_scores_backward_workspace_bytes(int N, int H, int B, int D) {
+}  // namespace d3f
+
+extern "C" size_t d3f_detection_scores_backward_workspace_bytes(int N, int H, int B, int D) {
   if (N < 0 || H < 0 || B < 1 || D < 1 || (long long)N * H >= (1ll << 31)) return 0;
   Carver cv(nullptr, 0);
   carve_det(cv, N, H, B, D);
   return cv.off + 1024;
 }
 
-int detection_scores_backward(const float* feats, const int* neighbors, const int* lengths, const float* dscores, int B,
-                              int N, int H, int D, float* dfeats, void* workspace, size_t workspace_bytes,
-                              cudaStream_t stream) {
+extern "C" int d3f_detection_scores_backward(const float* feats, const int* neighbors, const int* lengths,
+                                             const float* dscores, int B, int N, int H, int D, float* dfeats,
+                                             void* workspace, size_t workspace_bytes, d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(B >= 1 && B <= kMaxBatch && N >= 0 && H >= 0 && D >= 1, D3F_ERR_INVALID,
               "detection_scores_backward: bad shape B=%d N=%d H=%d D=%d", B, N, H, D);
   D3F_REQUIRE((long long)N * max(H, D) < (1ll << 31), D3F_ERR_INVALID,
               "detection_scores_backward: N*H or N*D beyond int32");
-  D3F_REQUIRE(workspace_bytes >= detection_scores_backward_workspace_bytes(N, H, B, D), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_detection_scores_backward_workspace_bytes(N, H, B, D), D3F_ERR_WORKSPACE,
               "detection_scores_backward: workspace too small");
   if (N == 0) return D3F_OK;
   D3F_REQUIRE(feats && (neighbors || H == 0) && lengths && dscores && dfeats && workspace, D3F_ERR_INVALID,
@@ -788,5 +817,3 @@ int detection_scores_backward(const float* feats, const int* neighbors, const in
   D3F_LAUNCH_CHECK("det_gather_kernel");
   return D3F_OK;
 }
-
-}  // namespace d3f

@@ -186,16 +186,22 @@ static size_t carve_voxel(Carver& cv, int N, int B, VoxelWs& w) {
   return cv.off;
 }
 
-size_t voxel_down_sample_workspace_bytes(int N, int B) {
+}  // namespace d3f
+
+using namespace d3f;
+
+extern "C" size_t d3f_voxel_down_sample_workspace_bytes(int N, int B) {
   if (N < 0 || B < 1 || B > kMaxBatch) return 0;
   Carver cv(nullptr, ~(size_t)0);
   VoxelWs w;
   return carve_voxel(cv, N, B, w) + 256;
 }
 
-int voxel_down_sample(const float* pts, const int* lengths, int B, int N, const int* n_dev, double voxel_size,
-                      const float* host_bbox, float* out_pts, int* out_lengths, int* out_M, int out_capacity,
-                      int* d_status, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+extern "C" int d3f_voxel_down_sample(const float* pts, const int* lengths, int B, int N, const int* n_dev,
+                                     double voxel_size, const float* host_bbox, float* out_pts, int* out_lengths,
+                                     int* out_M, int out_capacity, int* d_status, void* workspace,
+                                     size_t workspace_bytes, d3f_stream_t stream_) {
+  cudaStream_t stream = (cudaStream_t)stream_;
   D3F_REQUIRE(B >= 1 && B <= kMaxBatch, D3F_ERR_INVALID, "voxel_down_sample: B=%d must be in [1,%d]", B, kMaxBatch);
   D3F_REQUIRE(N >= 0, D3F_ERR_INVALID, "voxel_down_sample: N=%d", N);
   D3F_REQUIRE(isfinite(voxel_size) && voxel_size > 0.0, D3F_ERR_INVALID,
@@ -208,7 +214,7 @@ int voxel_down_sample(const float* pts, const int* lengths, int B, int N, const 
   for (int a = 0; a < 6; ++a)
     D3F_REQUIRE(isfinite(host_bbox[a]), D3F_ERR_INVALID, "voxel_down_sample: host_bbox[%d]=%g is not finite", a,
                 (double)host_bbox[a]);
-  D3F_REQUIRE(workspace_bytes >= voxel_down_sample_workspace_bytes(N, B), D3F_ERR_WORKSPACE,
+  D3F_REQUIRE(workspace_bytes >= d3f_voxel_down_sample_workspace_bytes(N, B), D3F_ERR_WORKSPACE,
               "voxel_down_sample: workspace too small");
   VoxelBits bits;
   bits.x = voxel_axis_bits((double)host_bbox[3] - (double)host_bbox[0], voxel_size);
@@ -253,5 +259,3 @@ int voxel_down_sample(const float* pts, const int* lengths, int B, int N, const 
   D3F_LAUNCH_CHECK("voxel_status_kernel");
   return D3F_OK;
 }
-
-}  // namespace d3f
