@@ -288,3 +288,223 @@ def d3feat_loss(desc, scores, anc, pos, points, config, weights, decisions=None)
         decisions["closest_negative_gap"] = float(((second - lo[:, 0]) / second).min())
         decisions["keypoint_score_gap"] = float(np.min(decisions["score_rows_gap"][np.concatenate([anc, pos])]))
     return desc_loss + det + reg, desc_loss, det, acc, fp.mean(), avg_neg
+
+
+# ----------------------------------------------------------------------------------------------------
+#  explicit adjoints with per-element magnitudes (tests/_oracle.assert_close)
+# ----------------------------------------------------------------------------------------------------
+# Each function evaluates an op's adjoint (and, for batch norm, its forward) on the fp32 inputs the kernel saw and
+# returns {name: (ref, mag)}: `mag` is the same computation summed over absolute values, the rounding-error scale of
+# that element. dtype=np.float32 gives the honest float32 evaluation tests/test_training_replay_oracle.py checks the
+# tolerance against. The branches the GPU decided on fp32 values are pinned to its choice: LeakyReLU's from the
+# recorded output (out > 0, the kernel's leaky_grad), max / min ties on the identical fp32 values both sides see.
+
+def _index_add(n_rows, index, values):
+    """float sum of values[i] into row index[i] of an [n_rows, C] zero array (numpy in, numpy out)."""
+    out = torch.zeros((n_rows,) + values.shape[1:], dtype=torch.from_numpy(values[:0]).dtype)
+    out.index_add_(0, torch.from_numpy(np.ascontiguousarray(index, np.int64)), torch.from_numpy(values))
+    return out.numpy()
+
+
+def _colsum(a, dt):
+    """Column sums accumulated in float64 and rounded to dt, as the kernels' float64 partials are."""
+    return a.sum(0, dtype=np.float64).astype(dt)
+
+
+def batch_norm_train_forward_ref(x, gamma, beta, residual=None, alpha=None, moving_mean=None, moving_var=None,
+                                 decay=None, eps=1e-6, dtype=np.float64):
+    """batch_norm_forward's out, batch mean, invstd and updated moving statistics: {name: (ref, mag)}. The output's
+    magnitude is |x*scale| + |beta| + |mean*scale| (+ |residual|): the apply pass is x*scale + shift with
+    shift = beta - mean*scale rounded on its own, and beta can cancel most of mean*scale."""
+    dt = dtype
+    x = np.asarray(x, dt)
+    b = np.asarray(beta, dt)
+    r = None if residual is None else np.asarray(residual, dt)
+    res = {}
+    if gamma is None:
+        y, m = x + b, np.abs(x) + np.abs(b)
+    else:
+        mean = _colsum(x, dt) / dt(x.shape[0])
+        var = _colsum(np.square(x - mean), dt) / dt(x.shape[0])
+        invstd = 1 / np.sqrt(var + dt(eps))
+        scale = np.asarray(gamma, dt) * invstd
+        shift = b - mean * scale
+        y, m = x * scale + shift, np.abs(x * scale) + np.abs(b) + np.abs(mean * scale)
+        res["mean"] = (mean, _colsum(np.abs(x), dt) / dt(x.shape[0]))
+        res["invstd"] = (invstd, invstd)
+        for k, stat, cur in (("moving_mean", mean, moving_mean), ("moving_var", var, moving_var)):
+            if cur is not None:
+                cur = np.asarray(cur, dt)
+                res[k] = (cur - (cur - stat) * dt(decay), np.abs(cur) + dt(decay) * (np.abs(cur) + np.abs(stat)))
+    if r is not None:
+        y, m = y + r, m + np.abs(r)
+    res["out"] = (y if alpha is None else np.where(y > 0, y, dt(alpha) * y), m)
+    return res
+
+
+def batch_norm_train_grads(x, out, dout, gamma, alpha=None, eps=1e-6, dtype=np.float64, mean=None, invstd=None):
+    """batch_norm_backward: {dres, dbeta (, dx, dgamma)}: (ref, mag), the LeakyReLU branch from the GPU's out.
+
+    mean / invstd: the batch statistics the backward is given (batch_norm_backward's inputs: the forward's float32
+    values); None computes them from x. xhat = (x - mean) * invstd is built from them, so a float32 mean, which moves
+    every xhat of a column by up to 2^-24 |mean| invstd (far more than |xhat| allows when |mean| >> std), is the
+    backward's input rather than its error. The forward check compares those statistics with float64 on their own.
+    Magnitudes: dbeta sum |dz|, dgamma sum |dz xhat|, dx |gamma invstd| (|dz| + sum |dz| / N + |xhat| sum |dz xhat| / N).
+    """
+    dt = dtype
+    x = np.asarray(x, dt)
+    N = x.shape[0]
+    dz = np.asarray(dout, dt)
+    if alpha is not None:
+        dz = np.where(np.asarray(out) > 0, dz, dt(alpha) * dz)
+    adz = np.abs(dz)
+    db, adb = _colsum(dz, dt), _colsum(adz, dt)
+    res = {"dres": (dz, adz), "dbeta": (db, adb)}
+    if gamma is None:
+        res["dx"] = (dz, adz)
+        return res
+    if mean is None:
+        mean = _colsum(x, dt) / dt(N)
+        invstd = 1 / np.sqrt(_colsum(np.square(x - mean), dt) / dt(N) + dt(eps))
+    mean, invstd = np.asarray(mean, dt), np.asarray(invstd, dt)
+    xh = (x - mean) * invstd
+    dg, adg = _colsum(dz * xh, dt), _colsum(np.abs(dz * xh), dt)
+    gi = np.asarray(gamma, dt) * invstd
+    res["dgamma"] = (dg, adg)
+    res["dx"] = (gi * (dz - db / dt(N) - xh * (dg / dt(N))),
+                 np.abs(gi) * (adz + adb / dt(N) + np.abs(xh) * (adg / dt(N))))
+    return res
+
+
+def ind_max_pool_grad(x, inds, dout, dtype=np.float64, chunk=4096):
+    """ind_max_pool_backward: (dx, mag). reduce_max splits a tie evenly over the tied entries; the shadow's shares go
+    through reduce_min to the rows equal to the column minimum, split evenly. mag: the sum of the absolute shares
+    routed to the element, the shadow's included."""
+    dt = dtype
+    x = np.asarray(x, dt)
+    g = np.asarray(dout, dt)
+    N1, C = x.shape
+    xs = np.concatenate([x, x.min(0, keepdims=True)], 0)
+    inds = np.asarray(inds, np.int64)
+    ii = np.where((inds < 0) | (inds >= N1), N1, inds)
+    acc, macc = np.zeros((N1 + 1, C), dt), np.zeros((N1 + 1, C), dt)
+    for a in range(0, ii.shape[0], chunk):
+        v = xs[ii[a:a + chunk]]                                            # [n, H, C]
+        tie = v == v.max(1, keepdims=True)
+        sh = np.where(tie, (g[a:a + chunk] / tie.sum(1))[:, None, :], dt(0)).reshape(-1, C)
+        flat = ii[a:a + chunk].reshape(-1)
+        acc += _index_add(N1 + 1, flat, sh)
+        macc += _index_add(N1 + 1, flat, np.abs(sh))
+    at_min = x == xs[N1][None]
+    n_min = at_min.sum(0)
+    return acc[:N1] + at_min * (acc[N1] / n_min), macc[:N1] + at_min * (macc[N1] / n_min)
+
+
+def gather_rows_grad(inds, dout, n_rows, dtype=np.float64):
+    """gather_rows_backward: (dx, mag), the sum of dout over each row's repeats; indices outside [0, n_rows) drop."""
+    g = np.asarray(dout, dtype)
+    inds = np.asarray(inds, np.int64)
+    ok = (inds >= 0) & (inds < n_rows)
+    return _index_add(n_rows, inds[ok], g[ok]), _index_add(n_rows, inds[ok], np.abs(g[ok]))
+
+
+def l2_normalize_grad(x, dout, eps=1e-10, dtype=np.float64):
+    """l2_normalize_backward: (dx, mag). sum x^2 >= eps (Maximum's tie goes to its first input): through the norm,
+    dx = (g - y (y.g)) inv, mag = (|g| + |y| sum |y g|) inv; below eps dx = g inv."""
+    dt = dtype
+    x, g = np.asarray(x, dt), np.asarray(dout, dt)
+    s = np.square(x).sum(1, keepdims=True)
+    through = s >= dt(eps)
+    inv = 1 / np.sqrt(np.maximum(s, dt(eps)))
+    y = x * inv
+    dx = np.where(through, (g - y * (y * g).sum(1, keepdims=True)) * inv, g * inv)
+    mag = np.where(through, (np.abs(g) + np.abs(y) * np.abs(y * g).sum(1, keepdims=True)) * inv, np.abs(g) * inv)
+    return dx, mag
+
+
+DET_MARGIN = 1e-5
+
+
+def detection_scores_grad(x, neighbors, lengths, gscore, dtype=np.float64, margin=DET_MARGIN, chunk=4096,
+                          parts=False):
+    """Explicit adjoint of detection_scores (the restatement above) for dL/dscore = gscore [N, 1]:
+    (dx, mag, alt, ambiguous rows). Per row, with f = x inv, mean = inv S / cnt (S = sum of the neighbour rows),
+    d = f - mean, e = 1e-6 + max_c f, ratio = f / e, p = softplus(d) ratio, score = max_c p:
+        dx[r] = gx[r] + sum over the entries (q, h) naming r of A[q] + (x[r] == M_b) share_b
+    gx = g_f inv (the direct path), A = -g_d inv / cnt (through the neighbour mean), share_b = -inv_b^2 sum over the
+    cloud's rows of dL/dinv, split over its elements equal to the cloud maximum M_b. mag: every term over absolute
+    values (|gx| + sum |A| + |share|, each from absolute products). The score's channel is the one decision fp32 can
+    take the other way: rows with a non-zero gradient whose two best channels lie within `margin` (relative) are
+    returned, and `alt` is the adjoint with each such row's second channel chosen instead. The channel maximum and the
+    cloud maximum are decided on the identical fp32 x and need no alternative. parts=True also returns the terms."""
+    dt = dtype
+    x = np.asarray(x, dt)
+    N, Dm = x.shape
+    gs = np.asarray(gscore, dt).reshape(N)
+    lengths = np.asarray(lengths, np.int64)
+    start = np.minimum(np.concatenate([[0], np.cumsum(lengths)]), N)
+    cloud = np.full(N, -1, np.int64)
+    inv = np.zeros(N, dt)
+    M = np.zeros(len(lengths), dt)
+    for b in range(len(lengths)):
+        a, e = int(start[b]), int(start[b + 1])
+        if e > a:
+            M[b] = x[a:e].max()
+            inv[a:e] = 1 / (M[b] + dt(1e-6))
+            cloud[a:e] = b
+    nb = np.asarray(neighbors, np.int64).reshape(N, -1)
+    valid = (nb >= 0) & (nb < N)
+    ii = np.where(valid, nb, N)
+    xs = np.concatenate([x, np.zeros((1, Dm), dt)], 0)
+    nz = np.concatenate([x.sum(1) != 0, [False]])
+    cnt = np.maximum((nz[ii] & valid).sum(1), 1).astype(dt)
+    S, Sa = np.zeros((N, Dm), dt), np.zeros((N, Dm), dt)
+    for a in range(0, N, chunk):
+        v = xs[ii[a:a + chunk]]
+        S[a:a + chunk], Sa[a:a + chunk] = v.sum(1), np.abs(v).sum(1)
+    f = x * inv[:, None]
+    mean = S * (inv / cnt)[:, None]
+    d = f - mean
+    dmax = f.max(1, keepdims=True)
+    e = dt(1e-6) + dmax
+    ratio = f / e
+    sp = np.where(d > 20, d, np.log1p(np.exp(np.minimum(d, dt(20)))))
+    sig = 1 / (1 + np.exp(-d))
+    p = sp * ratio
+    best = p.max(1, keepdims=True)
+    top = p == best
+    rest = np.where(top, -np.inf, p)
+    amb = (gs != 0) & ((best[:, 0] - rest.max(1)) <= dt(margin) * np.abs(best[:, 0]))
+    second = np.arange(Dm)[None, :] == rest.argmax(1)[:, None]
+    at_dmax = f == dmax
+    n_dmax = at_dmax.sum(1, keepdims=True)
+    at_M = (cloud >= 0)[:, None] & (x == M[np.maximum(cloud, 0)][:, None])
+    flat = ii.reshape(-1)
+    real = valid.reshape(-1)
+
+    def adjoint(sel, absolute):
+        ab = np.abs if absolute else (lambda t: t)
+        gp = np.where(sel, (gs / sel.sum(1))[:, None], dt(0))
+        gr, gd = gp * sp, gp * ratio * sig
+        gdm = -(ab(gr * f)).sum(1, keepdims=True) / e ** 2
+        gf = ab(gr / e) + at_dmax * ab(gdm / n_dmax) + ab(gd)
+        gx = ab(gf * inv[:, None])
+        A = ab(-gd * (inv / cnt)[:, None])
+        ginv = ab(gf * x).sum(1) + ab(-gd * S if not absolute else gd * Sa).sum(1) / cnt
+        share = np.zeros(len(lengths), dt)
+        for b in range(len(lengths)):
+            a, z = int(start[b]), int(start[b + 1])
+            if z > a:
+                tm = int(at_M[a:z].sum())
+                share[b] = ab(-ginv[a:z].sum() * inv[a] * inv[a] / tm)
+        spread = np.repeat(A, nb.shape[1], 0)[real] if nb.shape[1] else np.zeros((0, Dm), dt)
+        scat = _index_add(N, flat[real], spread)
+        sh = at_M * share[np.maximum(cloud, 0)][:, None]
+        return gx + scat + sh, dict(gx=gx, scatter=scat, share=sh, A=A)
+
+    ref, terms = adjoint(top, False)
+    mag, _ = adjoint(top, True)
+    sel2 = np.where(amb[:, None], second, top)
+    alt, _ = adjoint(sel2, False)
+    mag = np.maximum(mag, adjoint(sel2, True)[0])
+    return (ref, mag, alt, amb, terms) if parts else (ref, mag, alt, amb)

@@ -1,9 +1,13 @@
 """GPU: the training graph (d3feat_b200/training.py) against its float64 restatement (tests/_training_oracle.py).
 
-  * every new op's output and gradient within 1e-5 x mag (mag = largest |ref| of the tensor), the moving statistics
-    of batch norm too: batch norm with and without residual / LeakyReLU, the offset form, N = 1 and N = 0; the max
-    pool with ties, duplicate indices, shadow and -1 entries and an all-equal column; the row gather with repeats;
-    l2_normalize with rows below eps; detection scores with B = 1, 2, 5 and rows of no cloud;
+  * every new op's output and gradient element by element within TOL = 1e-5 x that element's magnitude of the
+    explicit float64 adjoints (_training_oracle: batch_norm_train_grads, ind_max_pool_grad, ...; _oracle.assert_close),
+    batch norm's batch statistics and moving statistics too: batch norm with and without residual / LeakyReLU, the
+    offset form, N = 1 and N = 0, N at the 2048-row partial blocks x C around the 32-column tiles, columns with
+    |mean| >> std; the max pool with ties, duplicate indices, shadow and -1 entries, an all-equal column, and shadow
+    entry counts at the 2048-entry partials; the row gather with repeats and one row gathered 1e5 times;
+    l2_normalize with rows below eps; detection scores with B = 1, 2, 5, rows of no cloud, a cloud of 7000 rows, a
+    cloud maximum tied across rows, and no neighbour columns;
   * the whole rigid network plus the loss on a seeded two-fragment batch: every parameter gradient within 3e-3 x its
     magnitude (TOL_NET says why not 1e-4), after checking that the seed's global decisions (cloud maxima, keypoint
     channel maxima, closest negatives) are far wider than the fp32 forward error;
@@ -16,6 +20,7 @@ import pytest
 import torch
 
 import _training_oracle as ot
+from _oracle import TOL, assert_close
 from oracle import kpconv_np as ok
 
 pytestmark = pytest.mark.gpu
@@ -46,65 +51,83 @@ def close(what, got, ref, tol, m=None):
     assert err <= tol, "%s: error %.3g x mag > %g" % (what, err, tol)
 
 
-def grads_of(fn_gpu, fn_ref, xs, dev, gout_seed=0):
-    """Outputs and input gradients of fn on the GPU (float32) and in the restatement (float64) for one seeded output
-    gradient."""
-    xs = [np.asarray(x, np.float32) for x in xs]              # both sides see the same float32 inputs
-    xg = [g(x, dev).requires_grad_(True) for x in xs]
-    xr = [ot.t64(x).requires_grad_(True) for x in xs]
-    yg, yr = fn_gpu(*xg), fn_ref(*xr)
-    go = np.random.default_rng(gout_seed).normal(size=tuple(yr.shape))
-    yg.backward(g(go, dev))
-    yr.backward(ot.t64(go))
-    return yg, yr, [a.grad for a in xg], [a.grad for a in xr]
+def grads_of(fn_gpu, xs, dev, gout_seed=0):
+    """fn's output and input gradients on the GPU (float32 inputs, as numpy) for one seeded output gradient, which is
+    returned too: (out, [dx...], gout)."""
+    xg = [g(np.asarray(x, np.float32), dev).requires_grad_(True) for x in xs]
+    y = fn_gpu(*xg)
+    go = np.random.default_rng(gout_seed).normal(size=tuple(y.shape)).astype(np.float32)
+    y.backward(g(go, dev))
+    return y.detach().cpu().numpy(), [a.grad.cpu().numpy() for a in xg], go
 
 
 # ---------------------------------------------------------------------------------------------------- ops
+# Every op's output and gradients element by element against the explicit float64 adjoints of _training_oracle
+# (ref, mag): |gpu - ref| <= TOL * mag (tests/_oracle.py).
 
-@pytest.mark.parametrize("N,C,res,alpha", [(5000, 64, False, 0.2), (3000, 128, True, 0.2), (2100, 32, True, None),
-                                           (1, 16, False, 0.2), (4097, 3, False, None)])
-def test_batch_norm(cuda, N, C, res, alpha):
+def check_batch_norm(dev, x, res, alpha, seed=0, what="bn"):
     from d3feat_b200 import training as T
-    rng = np.random.default_rng(N + C)
-    x = rng.normal(size=(N, C)) * rng.uniform(0.5, 3, C) + rng.normal(size=C)
-    gm, bt = rng.uniform(0.5, 1.5, C), rng.normal(size=C) * 0.1
-    r = rng.normal(size=(N, C)) if res else None
-    mm, mv = rng.normal(size=C) * 0.1, rng.uniform(0.5, 1.5, C)
-    mmg, mvg = g(mm, cuda), g(mv, cuda)
+    N, C = x.shape
+    rng = np.random.default_rng(seed)
+    x = np.float32(x)
+    gm, bt = np.float32(rng.uniform(0.5, 1.5, C)), np.float32(rng.normal(size=C) * 0.1)
+    r = np.float32(rng.normal(size=(N, C))) if res else None
+    mm, mv = np.float32(rng.normal(size=C) * 0.1), np.float32(rng.uniform(0.5, 1.5, C))
+    mmg, mvg = g(mm, dev), g(mv, dev)
 
     def gpu(x, gm, bt, *r):
         return T._BatchNormFn.apply(x, gm, bt, r[0] if r else None, mmg, mvg, 0.98, alpha)
 
-    def ref(x, gm, bt, *r):
-        return ot.batch_norm_train(x, gm, bt, r[0] if r else None, alpha)[0]
+    out, grads, go = grads_of(gpu, [x, gm, bt] + ([r] if res else []), dev, seed)
+    fw = ot.batch_norm_train_forward_ref(x, gm, bt, r, alpha, mm, mv, float(np.float32(1 - 0.98)))
+    assert_close(out, *fw["out"], what=what + " out")
+    assert_close(mmg.cpu(), *fw["moving_mean"], what=what + " moving_mean")
+    assert_close(mvg.cpu(), *fw["moving_var"], what=what + " moving_var")
+    # the batch statistics the backward reads (the forward is deterministic: the same bits as the step's)
+    _, mean, invstd = T.batch_norm_forward(g(x, dev), g(gm, dev), g(bt, dev), g(mm, dev), g(mv, dev), 0.98)
+    mean, invstd = mean.cpu().numpy(), invstd.cpu().numpy()
+    assert_close(mean, *fw["mean"], what=what + " mean")
+    assert_close(invstd, *fw["invstd"], what=what + " invstd")
+    bw = ot.batch_norm_train_grads(x, out, go, gm, alpha, mean=mean, invstd=invstd)
+    for n, got in zip(["dx", "dgamma", "dbeta", "dres"], grads):
+        assert_close(got, *bw[n], what=what + " " + n)
 
-    ins = [x, gm, bt] + ([r] if res else [])
-    yg, yr, dg, dr = grads_of(gpu, ref, ins, cuda)
-    _, mean, var = ot.batch_norm_train(ot.t64(np.float32(x)), ot.t64(gm), ot.t64(bt))
-    # out = x*inv + (beta - mean*inv) (+ r): its rounding scale is |x*inv| + |beta - mean*inv| (+ |r|), which is far
-    # above |out| when the batch variance is small (N = 1: inv = gamma * 1000); dx scales with |inv| |dout|
-    inv = (ot.t64(gm) / torch.sqrt(var + 1e-6)).numpy()
-    xf = np.float32(x).astype(np.float64)
-    m_out = np.abs(xf * inv) + np.abs(bt - mean.numpy() * inv) + (np.abs(r) if res else 0)
-    go = np.random.default_rng(0).normal(size=(N, C))
-    close("bn out", yg, yr, TOL_OP, m_out.max())
-    close("bn dx", dg[0], dr[0], TOL_OP, max(np.abs(dr[0].numpy()).max(), (np.abs(inv) * np.abs(go).max()).max()))
-    for n, a, b in zip(["dgamma", "dbeta", "dres"], dg[1:], dr[1:]):
-        close("bn " + n, a, b, TOL_OP)
-    f32 = lambda a: ot.t64(np.float32(a))
-    close("bn moving_mean", mmg, f32(mm) - (f32(mm) - mean) * 0.02, TOL_OP)
-    close("bn moving_var", mvg, f32(mv) - (f32(mv) - var) * 0.02, TOL_OP)
+
+@pytest.mark.parametrize("N,C,res,alpha", [(5000, 64, False, 0.2), (3000, 128, True, 0.2), (2100, 32, True, None),
+                                           (1, 16, False, 0.2), (4097, 3, False, None)])
+def test_batch_norm(cuda, N, C, res, alpha):
+    rng = np.random.default_rng(N + C)
+    x = rng.normal(size=(N, C)) * rng.uniform(0.5, 3, C) + rng.normal(size=C)
+    check_batch_norm(cuda, x, res, alpha, N + C)
+
+
+@pytest.mark.parametrize("N", [2047, 2048, 2049, 3 * 2048 + 1])
+@pytest.mark.parametrize("C", [1, 31, 33, 256])
+def test_batch_norm_block_boundaries(cuda, N, C):
+    """N at the 2048-row blocks of colsum_partial_kernel's partials, C around its 32-column tiles."""
+    rng = np.random.default_rng(N * 7 + C)
+    x = rng.normal(size=(N, C)) * rng.uniform(0.5, 3, C) + rng.normal(size=C)
+    check_batch_norm(cuda, x, (N + C) % 2 == 1, 0.2 if C != 33 else None, N + C, "bn %dx%d" % (N, C))
+
+
+@pytest.mark.parametrize("N,C", [(6145, 64), (2049, 33)])
+def test_batch_norm_mean_far_above_std(cuda, N, C):
+    """x = 1e3 + N(0, 1): x - mean cancels 10 bits; the variance, xhat and dx must not lose them. The output gradient
+    is the centred x itself (the same draws), so dgamma / N is of order one and xhat's error reaches dx."""
+    rng = np.random.default_rng(N)
+    check_batch_norm(cuda, 1e3 + rng.normal(size=(N, C)), True, 0.2, N, "bn mean>>std %dx%d" % (N, C))
 
 
 def test_batch_norm_offset_and_empty(cuda):
     from d3feat_b200 import training as T
     rng = np.random.default_rng(3)
-    x, off, r = rng.normal(size=(700, 24)), rng.normal(size=24), rng.normal(size=(700, 24))
-    yg, yr, dg, dr = grads_of(lambda x, o, r: T._BatchNormFn.apply(x, None, o, r, None, None, 0.98, 0.2),
-                              lambda x, o, r: ot.batch_norm_train(x, None, o, r, 0.2)[0], [x, off, r], cuda)
-    close("offset out", yg, yr, TOL_OP)
-    for n, a, b in zip(["dx", "doffset", "dres"], dg, dr):
-        close("offset " + n, a, b, TOL_OP)
+    x, off, r = (np.float32(a) for a in (rng.normal(size=(700, 24)), rng.normal(size=24), rng.normal(size=(700, 24))))
+    out, grads, go = grads_of(lambda x, o, r: T._BatchNormFn.apply(x, None, o, r, None, None, 0.98, 0.2), [x, off, r],
+                              cuda)
+    assert_close(out, *ot.batch_norm_train_forward_ref(x, None, off, r, 0.2)["out"], what="offset out")
+    bw = ot.batch_norm_train_grads(x, out, go, None, 0.2)
+    for n, got in zip(["dx", "dbeta", "dres"], grads):
+        assert_close(got, *bw[n], what="offset " + n)
     # N = 0: empty output, moving statistics untouched, zero dgamma / dbeta
     mm, mv = torch.full((8,), 0.5, device=cuda), torch.full((8,), 2.0, device=cuda)
     gm = torch.ones(8, device=cuda, requires_grad=True)
@@ -129,14 +152,40 @@ def pool_case(rng, N1=900, N2=400, H=12, C=40):
     return x, inds
 
 
+def check_pool(dev, x, inds, what):
+    from d3feat_b200 import training as T
+    ig = g(inds, dev, torch.int32)
+    out, (dx,), go = grads_of(lambda x: T._MaxPoolFn.apply(x, ig), [x], dev)
+    assert np.array_equal(out, ot.ind_max_pool(ot.t64(x), inds).numpy())      # a selection: exact
+    assert_close(dx, *ot.ind_max_pool_grad(x, inds, go), what=what)
+
+
 @pytest.mark.parametrize("seed", [0, 1])
 def test_ind_max_pool(cuda, seed):
-    from d3feat_b200 import training as T
     x, inds = pool_case(np.random.default_rng(seed))
-    ig = g(inds, cuda, torch.int32)
-    yg, yr, dg, dr = grads_of(lambda x: T._MaxPoolFn.apply(x, ig), lambda x: ot.ind_max_pool(x, inds), [x], cuda)
-    close("pool out", yg, yr, TOL_OP)
-    close("pool dx", dg[0], dr[0], TOL_OP)
+    check_pool(cuda, x, inds, "pool dx seed %d" % seed)
+
+
+@pytest.mark.parametrize("N2,H,n_shadow", [(91, 45, 2047), (91, 45, 2049), (128, 16, 2048), (241, 17, 4097),
+                                           (683, 3, 2049)])
+def test_ind_max_pool_shadow_blocks(cuda, N2, H, n_shadow):
+    """N2*H (4095, 4097, 2048, 2049) and the number of shadow entries just below, at and above multiples of 2048:
+    shadow_partial_kernel sums the shadow's gradient in 2048-entry partials. The all-shadow rows come last, so the
+    last partial holds gradient the column minimum must receive."""
+    rng = np.random.default_rng(N2 + H + n_shadow)
+    N1, C = 700, 36
+    x = rng.normal(size=(N1, C)).astype(np.float32)
+    x[::9, 2] = x[:, 2].min()
+    inds = rng.integers(0, N1, size=(N2, H)).astype(np.int32)
+    full, extra = divmod(min(n_shadow, N2 * H), H)
+    flat = inds.reshape(-1)
+    flat[N2 * H - full * H:] = N1                              # the last `full` rows: shadow only
+    head = N2 * H - full * H
+    if extra:
+        pick = rng.choice(head, extra, replace=False)
+        flat[pick] = np.where(pick % 2 == 0, N1, -1)           # the rest of the shadow entries, some of them -1
+    assert int(((inds < 0) | (inds >= N1)).sum()) == min(n_shadow, N2 * H)
+    check_pool(cuda, x, inds, "pool shadow %dx%d/%d" % (N2, H, n_shadow))
 
 
 def test_gather_rows(cuda):
@@ -147,9 +196,20 @@ def test_gather_rows(cuda):
     inds[::9] = 3000                                           # shadow: zero row, gradient dropped
     inds[:300] = 17                                            # one row gathered 300 times
     ig = g(inds, cuda, torch.int32)
-    yg, yr, dg, dr = grads_of(lambda x: T._GatherFn.apply(x, ig), lambda x: ot.gather_rows(x, inds), [x], cuda)
-    close("gather out", yg, yr, TOL_OP)
-    close("gather dx", dg[0], dr[0], TOL_OP)
+    out, (dx,), go = grads_of(lambda x: T._GatherFn.apply(x, ig), [x], cuda)
+    assert np.array_equal(out, ot.gather_rows(ot.t64(np.float32(x)), inds).numpy())
+    assert_close(dx, *ot.gather_rows_grad(inds, go, 3000), what="gather dx")
+
+
+def test_gather_one_row_1e5_times(cuda):
+    from d3feat_b200 import training as T
+    rng = np.random.default_rng(15)
+    x = rng.normal(size=(500, 32))
+    inds = rng.integers(0, 500, size=120000).astype(np.int32)
+    inds[rng.choice(120000, 100000, replace=False)] = 42       # row 42 gathered 1e5 times, interleaved
+    ig = g(inds, cuda, torch.int32)
+    _, (dx,), go = grads_of(lambda x: T.gather_rows(x, ig), [x], cuda)
+    assert_close(dx, *ot.gather_rows_grad(inds, go, 500), what="gather 1e5 repeats dx")
 
 
 def test_l2_normalize(cuda):
@@ -157,9 +217,11 @@ def test_l2_normalize(cuda):
     rng = np.random.default_rng(6)
     x = rng.normal(size=(4000, 32))
     x[::13] *= 1e-7                                            # sum x^2 below eps = 1e-10
-    yg, yr, dg, dr = grads_of(T.l2_normalize, ot.l2_normalize, [x], cuda)
-    close("l2 out", yg, yr, TOL_OP)
-    close("l2 dx", dg[0], dr[0], TOL_OP)
+    out, (dx,), go = grads_of(T.l2_normalize, [x], cuda)
+    xf = np.float32(x)
+    assert_close(out, ot.l2_normalize(ot.t64(xf)).numpy(), np.abs(ot.l2_normalize(ot.t64(np.abs(xf))).numpy()),
+                 what="l2 out")
+    assert_close(dx, *ot.l2_normalize_grad(xf, go), what="l2 dx")
 
 
 def det_case(rng, lengths, N, H=20, D=32):
@@ -175,16 +237,45 @@ def det_case(rng, lengths, N, H=20, D=32):
     return x, nb
 
 
+def check_det(dev, x, nb, lengths, what):
+    from d3feat_b200 import training as T
+    N = x.shape[0]
+    nbg, lg = g(nb, dev, torch.int32), g(np.asarray(lengths, np.int32), dev, torch.int32)
+    out, (dx,), go = grads_of(lambda x: T.detection_scores(x, nbg, lg), [x], dev)
+    xf = np.float32(x)
+    rows = min(N, sum(lengths))                                # rows past the last cloud: unspecified score
+    ref = ot.detection_scores(ot.t64(xf), nb, lengths).numpy()
+    assert np.all(np.abs(out[:rows] - ref[:rows]) <= TOL * np.abs(ref[:rows]).max())
+    ref, mag, alt, amb = ot.detection_scores_grad(xf, nb, lengths, go)
+    print("%s: %d of %d rows checked against both channels" % (what, int(amb.sum()), N))
+    assert amb.sum() <= max(1, 1e-3 * N)
+    assert_close(dx, ref, mag, what=what, alt=alt)
+
+
 @pytest.mark.parametrize("lengths,N", [([2500], 2500), ([1200, 1300], 2500), ([500, 700, 0, 900, 300], 2600)])
 def test_detection_scores(cuda, lengths, N):
-    from d3feat_b200 import training as T
     x, nb = det_case(np.random.default_rng(len(lengths)), lengths, N)
-    nbg, lg = g(nb, cuda, torch.int32), g(np.asarray(lengths, np.int32), cuda, torch.int32)
-    yg, yr, dg, dr = grads_of(lambda x: T.detection_scores(x, nbg, lg),
-                              lambda x: ot.detection_scores(x, nb, lengths), [x], cuda)
-    rows = min(N, sum(lengths))                                # rows past the last cloud: unspecified score
-    close("det out", yg[:rows], yr[:rows], TOL_OP)
-    close("det dx", dg[0], dr[0], TOL_OP)
+    check_det(cuda, x, nb, lengths, "det dx B=%d" % len(lengths))
+
+
+def test_detection_scores_large_cloud_and_tied_maximum(cuda):
+    """A 7000-row cloud (det_cloud_grad_kernel sums its dL/dinv in 2048-row chunks) next to a 2100-row one, each
+    with its maximum tied across several rows."""
+    lengths = [7000, 2100]
+    rng = np.random.default_rng(21)
+    x, nb = det_case(rng, lengths, sum(lengths))
+    for a, e, rows in ((0, 7000, [5, 2048, 4097, 6999]), (7000, 9100, [7001, 9099])):
+        m = x[a:e].max() + 0.5
+        for i, r in enumerate(rows):
+            x[r, i % 32] = m
+    check_det(cuda, x, nb, lengths, "det dx large cloud, tied max")
+
+
+def test_detection_scores_no_neighbours(cuda):
+    """H = 0: every mean is zero (count clamped to 1), nothing is scattered."""
+    lengths = [1500, 1100]
+    x, _ = det_case(np.random.default_rng(22), lengths, 2600)
+    check_det(cuda, x, np.zeros((2600, 0), np.int32), lengths, "det dx H=0")
 
 
 # ---------------------------------------------------------------------------------------------------- network
