@@ -1230,7 +1230,11 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
     const int rc = kpconv_prep_supports(deform, s, feat, Ns, ns_dev, K, Cin, normalize, s4, stream);
     if (rc) return rc;
   }
-  if (Cin == 1 && !deform && K == 15) {
+  // The first-layer kernel stages W[K, Cout] and Kp in 48 KB of shared memory: Cout <= 816. A wider Cin = 1 layer (or
+  // the feature gradient of a Cout = 1 layer, whose transposed problem has Cin = 1) runs the two-stage path below;
+  // its support pack then holds the feature itself, and the `> 0` test of stage 1's count is the same predicate.
+  const size_t c1_smem = (size_t)(K * Cout + K * 3) * sizeof(float);
+  if (Cin == 1 && !deform && K == 15 && c1_smem <= 48 * 1024) {
     Cin1Params c1;
     c1.q = q; c1.s4 = s4; c1.idx = idx; c1.Kp = Kp; c1.W = W;
     c1.Nq = Nq; c1.Ns = Ns; c1.H = H; c1.Cout = Cout;
@@ -1243,8 +1247,6 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
     c1.order = query_order;
     c1.out = out;
     c1.nq_dev = nq_dev; c1.ns_dev = ns_dev;
-    const size_t c1_smem = (size_t)(K * Cout + K * 3) * sizeof(float);
-    D3F_REQUIRE(c1_smem <= 48 * 1024, D3F_ERR_CAPACITY, "kpconv (Cin = 1): Cout=%d too wide for the first-layer kernel", Cout);
     if (influence == D3F_INFLUENCE_LINEAR && mode == D3F_MODE_SUM)
       kpconv_cin1_kernel<true><<<ceil_div(ceil_div(Nq, 4) * 32, 256), 256, c1_smem, stream>>>(c1);
     else

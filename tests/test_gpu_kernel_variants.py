@@ -5,9 +5,10 @@ launch_stage1 (kpconv.cu) and tc_gemm / gemm_f32 pick among many template instan
 influence, mode, K and the number of rows. The table below names the instance each case must reach, so a dispatch
 change that moves a case off its kernel fails here instead of silently dropping that kernel from the suite.
 
-Not reachable in a normal process and therefore not in the table: kpconv_stage1_mma_kernel<NT, false, true> (rigid
-linear-sum with the 64-channel-pass kernels switched off by D3F_S1_PARED=0, read once per process), and split-K with a
-residual (only the KPConv contraction splits K, and it has no residual).
+Not in the table: kpconv_stage1_mma_kernel<NT, false, true> (rigid linear-sum with the 64-channel-pass kernels
+switched off by D3F_S1_PARED=0, which is read once per process: tests/test_gpu_grad_variants.py runs it forward and
+backward in a child process), and split-K with a residual (not reachable: only the KPConv contraction splits K, and it
+has no residual).
 
 The multi-chunk KPConv pipeline (chunks of D3F_KPCONV_CHUNK queries; the variable is read once per process) runs in a
 child process at two chunk sizes.
@@ -209,12 +210,18 @@ def test_kpconv_variant(cuda, monkeypatch, c):
     assert_close(out, ref, mag, TOL, "kpconv " + c["id"], alt=alt)
 
 
-def test_kpconv_cin1_cout817_does_not_fit(cuda):
+def test_kpconv_cin1_cout817_runs_two_stage(cuda):
+    """Cin = 1 with W[15, 817] past the first-layer kernel's 48 KB: the generic stage 1 and the CUDA-core contraction
+    (K * Cin = 15) run instead, with the same normalisation."""
     from d3feat_b200 import convolution_ops as co
-    from d3feat_b200._lib import D3FError
     q, s, idx, f, Kp, W = make_case(np.random.default_rng(1), 200, 200, 20, 1, 817)
-    with pytest.raises(D3FError):
-        co.KPConv_ops(t(q, cuda), t(s, cuda), t(idx, cuda), t(f, cuda), t(Kp, cuda), t(W, cuda), 0.06, "linear", "sum")
+    f[::3] = -np.abs(f[::3])              # supports that do not count towards nn
+    out, names = launched(lambda: co.KPConv_ops(t(q, cuda), t(s, cuda), t(idx, cuda), t(f, cuda), t(Kp, cuda),
+                                                t(W, cuda), 0.06, "linear", "sum"))
+    assert_ran(names, [GENERIC, F32])
+    assert not any("kpconv_cin1_kernel" in n for n in names)
+    ref, mag, alt = kpconv_ref(q, s, idx, f, Kp, W, 0.06)
+    assert_close(out.cpu().numpy(), ref, mag, TOL, "kpconv cin1 cout817", alt=alt)
 
 
 # ---- edges, on each stage-1 family ----------------------------------------------------------------------------------

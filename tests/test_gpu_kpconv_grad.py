@@ -239,9 +239,17 @@ def _no_grad_check(launched):
     counted = launched
 
     def launched(fn):
-        c0 = _lib.launch_count()
-        out, names = counted(fn)
-        return out, (names, _lib.launch_count() - c0)
+        # the library's launch count of the call whose kernels were captured: the profiler repeats the call when a
+        # capture comes back empty, and the earlier attempts must not add to it
+        calls = []
+
+        def one_call():
+            c0 = _lib.launch_count()
+            out = fn()
+            calls.append(_lib.launch_count() - c0)
+            return out
+        out, names = counted(one_call)
+        return out, (names, calls[-1])
     rng = np.random.default_rng(12)
     for Cin, Cout in ((1, 64), (32, 32), (64, 64), (48, 40)):
         q, s, idx, f, Kp, W, _ = make_case(rng, 2000, 2000, 40, Cin, Cout, extent=0.08)
