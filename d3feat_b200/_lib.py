@@ -84,6 +84,9 @@ SYMBOLS = [
     ("d3f_evaluate_pairs_workspace_bytes", _Z, [_I, _I]),
     ("d3f_evaluate_pairs", _I, [_P, _P, _I, _I, _P, _P, _I, _P, _I, _P, _P, _P, _P, _I, _P, _I, _D, _D, _D, _D, _D, _D,
                                 _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _Z, _P]),
+    ("d3f_momentum_clip_workspace_bytes", _Z, [_I, _LL]),
+    ("d3f_momentum_clip_update", _I, [_P, _I, _LL, _F, _F, _F, _P, _Z, _P]),
+    ("d3f_rank_mean", _I, [_P, _I, _LL, _P, _P]),
 ]
 
 _lib = None

@@ -12,7 +12,7 @@ _STAMP = os.path.join(_HERE, "csrc", ".build_stamp")
 
 SOURCES = ["api.cu", "sort.cu", "grid.cu", "neighbors.cu", "kpconv.cu", "kpconv_fused.cu", "gemm.cu", "pool.cu", "tc_gemm.cu", "pyramid.cu",
            "keypoints.cu", "matching.cu", "registration.cu", "icp.cu", "evaluation.cu", "voxel.cu", "kpconv_grad.cu", "train_ops.cu",
-           "correspond.cu"]
+           "correspond.cu", "optim.cu"]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--expt-relaxed-constexpr"]

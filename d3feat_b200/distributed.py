@@ -2,9 +2,17 @@
 ONE all-gather of the per-fragment descriptors at the end (NCCL over NVLink/NVSwitch between H100s, gloo in
 the CPU tests). The reference is single-process (SURVEY.md 8e): fragments are independent units, so there is no
 data-path collective inside the pyramid or the encoder.
+
+Data-parallel training: each rank runs training.forward / d3feat_loss / backward on its own pair, then
+reduce_gradients, the update (training.MomentumClip) and reduce_moving_statistics. Both reductions all-gather the
+ranks' values and take their mean in rank order in fp64 (d3f_rank_mean): an all-gather only copies, so, unlike
+all_reduce, whose summation order depends on NCCL's algorithm and the topology, the result is the same bits on every
+rank, run to run and for any topology.
 """
 import torch
 import torch.distributed as dist
+
+from . import _lib
 
 
 def shard_fragments(n_fragments, rank, world_size):
@@ -102,3 +110,87 @@ def all_gather_descriptors(local_desc, local_rows_per_fragment, group=None):
     rows_t = torch.tensor(list(local_rows_per_fragment), dtype=torch.int64, device=dev).reshape(-1)
     gathered, metas = all_gather_descriptors_padded(local_desc, rows_t, max(cap, 1), group, max_fragments=max(fmax, 1))
     return unpack_gathered(gathered, metas)
+
+
+# ----------------------------------------------------------------------------------------------------
+#  data-parallel training
+# ----------------------------------------------------------------------------------------------------
+
+def rank_mean(x, out=None):
+    """x float32 [R, P] (CUDA) -> out [P] = fl32((x[0] + ... + x[R-1]) / R), summed in fp64 in rank order
+    (d3f_rank_mean; oracle/optim_np.rank_mean). R = 1 returns x[0]'s bits. out may be x[0]."""
+    op = "rank_mean"
+    x = _lib.tensor_arg(x, op + ": x", torch.float32, (None, None))
+    R, P = x.shape
+    if R < 1:
+        raise ValueError("%s: x has no ranks" % op)
+    if out is None:
+        out = torch.empty((P,), dtype=torch.float32, device=x.device)
+    elif not (torch.is_tensor(out) and out.is_contiguous()):
+        raise ValueError("%s: out must be a contiguous tensor (it is written in place)" % op)
+    out = _lib.tensor_arg(out, op + ": out", torch.float32, (P,), x.device)
+    _lib.check(_lib.lib().d3f_rank_mean(_lib.ptr(x), R, P, _lib.ptr(out), _lib.stream()), "d3f_rank_mean")
+    return out
+
+
+def _gather_rows(flat, group):
+    """[R, P]: every rank's flat float32 buffer, in rank order. Without a process group: flat as [1, P]."""
+    if not dist.is_available() or not dist.is_initialized():
+        return flat.view(1, -1)
+    out = torch.empty((dist.get_world_size(group), flat.numel()), dtype=flat.dtype, device=flat.device)
+    if dist.get_backend(group) == "nccl":
+        dist.all_gather_into_tensor(out.view(-1), flat, group=group)
+    else:
+        dist.all_gather(list(out.unbind(0)), flat, group=group)
+    return out
+
+
+def _mean_over_ranks(tensors, group):
+    """Replace every tensor's values by their mean over the ranks (rank order, fp64), in place."""
+    if not tensors:
+        return
+    flat = torch.cat([t.detach().reshape(-1) for t in tensors])
+    mean = rank_mean(_gather_rows(flat, group), out=flat)
+    views = [m.view(t.shape) for m, t in zip(mean.split([t.numel() for t in tensors]), tensors)]
+    with torch.no_grad():
+        torch._foreach_copy_(tensors, views)        # one launch for all tensors, not one per tensor
+
+
+def reduce_gradients(params, group=None):
+    """Data-parallel gradient: every parameter's .grad becomes the mean of the ranks' gradients, taken in rank order
+    in fp64 (rank_mean) over one all-gather of all gradients, so every rank holds the same bits. With one pair per
+    rank this is the gradient of the mean of the ranks' losses. A parameter without a gradient counts as zero (its
+    .grad is created), so a rank whose pair was skipped still takes part. Every rank must pass the same parameters in
+    the same order. No host synchronisation (the collective is enqueued on the current stream)."""
+    params = list(params)
+    for i, p in enumerate(params):
+        _lib.tensor_arg(p, "reduce_gradients: params[%d]" % i, torch.float32)
+        if p.grad is None:
+            p.grad = torch.zeros_like(p, memory_format=torch.contiguous_format)
+        else:
+            _lib.tensor_arg(p.grad, "reduce_gradients: params[%d].grad" % i, torch.float32, tuple(p.shape), p.device)
+    _mean_over_ranks([p.grad for p in params], group)
+
+
+def reduce_moving_statistics(store, group=None):
+    """Replace every moving_mean / moving_variance of the ParamStore by its mean over the ranks (rank_mean, in
+    place), so that every replica holds the same store and writes the same snapshot. Call it after each step: each
+    rank's batch norm updated its own statistics from its own pair."""
+    names = [n for n in sorted(store.t) if n.rsplit("/", 1)[-1] in ("moving_mean", "moving_variance")]
+    for n in names:
+        _lib.tensor_arg(store.t[n], "reduce_moving_statistics: " + n, torch.float32)
+    _mean_over_ranks([store.t[n] for n in names], group)
+
+
+STEP_STATS = ("loss", "desc_loss", "det_loss", "accuracy", "d_pos", "d_neg")
+
+
+def gather_step_stats(stats, group=None):
+    """[R, 6] float32 on the device: every rank's (loss, desc_loss, det_loss, accuracy, d_pos, d_neg), the values
+    training.d3feat_loss returns, in rank order (for logging; no host synchronisation)."""
+    stats = list(stats)
+    if len(stats) != len(STEP_STATS):
+        raise ValueError("gather_step_stats: %d values, expected the %d of d3feat_loss %s" % (
+            len(stats), len(STEP_STATS), STEP_STATS))
+    flat = torch.stack([v.detach().reshape(()).to(torch.float32) for v in stats])
+    return _gather_rows(flat, group).clone()

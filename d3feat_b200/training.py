@@ -3,25 +3,27 @@ models/D3Feat.py with training = True, and the loss of models/KPFCNN_model.py:14
 
     store = ParamStore(params, "cuda")
     params = training.trainable(store)               # weights, gamma, beta, offset require grad
-    opt = torch.optim.SGD(params, lr=config.learning_rate, momentum=config.momentum)
+    opt = training.MomentumClip(params, config.learning_rate, config.momentum, config.grad_clip_norm)
     with use_params(store):
         desc, scores = training.forward(inputs, config)       # inputs: exact-shape pyramid (pyramid.descriptor_input)
         loss, *stats = training.d3feat_loss(desc, scores, anc_inds, pos_inds, points, config)
     opt.zero_grad(); loss.backward()
-    for p in params: torch.nn.utils.clip_grad_norm_([p], config.grad_clip_norm)   # tf.clip_by_norm, per gradient
-    opt.step()
+    opt.step()                                       # tf.clip_by_norm per gradient + tf.train.MomentumOptimizer
 
 The differentiable ops are torch.autograd.Functions over sm_90a kernels (train_ops.cu): batch norm in training mode
 (batch statistics, moving-average update in place), ind_max_pool, closest_pool / gather_rows, l2_normalize and
-detection_scores. The convolutions are the differentiable conv_ops.KPConv / unary_convolution. The inference path
-(network_blocks, encoder.KPFCNN) is untouched and still refuses training = True; because the moving statistics are
-updated in place, ParamStore.bn_affine picks the trained statistics up. The loss is small tensor algebra on the
+detection_scores. The update is MomentumClip over optim.cu. The convolutions are the differentiable conv_ops.KPConv /
+unary_convolution. The inference path (network_blocks, encoder.KPFCNN) is untouched and still refuses
+training = True; because the moving statistics are updated in place, ParamStore.bn_affine picks the trained
+statistics up. The loss is small tensor algebra on the
 keypoints and stays in torch.
 
 The step is not graph-capturable (the KPConv feature gradient reads its reverse width back to the host), so inputs
 must have exact shapes: a static (capacity-sized) pyramid is refused with ValueError. Deformable blocks have no
 gradient here and raise NotImplementedError.
 """
+import types
+
 import numpy as np
 import torch
 import torch.nn.functional as Fn
@@ -36,8 +38,10 @@ BN_EPSILON = 1e-6        # models/network_blocks.py:155
 L2_EPSILON = 1e-10       # tf.nn.l2_normalize default (models/D3Feat.py:65)
 
 # training_3DMatch.py:79-113 (weights_decay: utils/config.py:137)
+# lr_decays (:107) is read-only: every Config built from these dicts shares it (assign a new dict to change it)
 TRAINING_3DMATCH = dict(batch_norm_momentum=0.98, learning_rate=1e-1, momentum=0.98, grad_clip_norm=100.0,
-                        weights_decay=1e-6, det_loss_weight=1.0, safe_radius=0.1, keypts_num=256)
+                        weights_decay=1e-6, det_loss_weight=1.0, safe_radius=0.1, keypts_num=256,
+                        lr_decays=types.MappingProxyType({i: 0.1 ** (1 / 80) for i in range(1, 200)}))
 # training_KITTI.py:63-113
 TRAINING_KITTI = dict(TRAINING_3DMATCH, first_subsampling_dl=0.30, safe_radius=1.0, keypts_num=1024)
 
@@ -510,3 +514,130 @@ def d3feat_loss(descriptors, scores, anc_inds, pos_inds, backup_points, config):
     else:
         det_loss = torch.zeros((), dtype=dists.dtype, device=dists.device)
     return desc_loss + det_loss + reg, desc_loss, det_loss, accuracy, d_pos, d_neg
+
+
+# ----------------------------------------------------------------------------------------------------
+#  the update (utils/trainer.py:116-156, 376-381)
+# ----------------------------------------------------------------------------------------------------
+
+def learning_rate(config, epoch):
+    """The learning rate during epoch `epoch` (0-based) of the reference's trainer: a float32 variable that starts at
+    config.learning_rate and, at the end of every epoch e in config.lr_decays, is assigned fl32(lr * fl32(decay))
+    (utils/trainer.py:376-381). No lr_decays: no decay."""
+    lr = np.float32(config.learning_rate)
+    decays = getattr(config, "lr_decays", None) or {}
+    for e in range(int(epoch)):
+        if e in decays:
+            lr = lr * np.float32(decays[e])
+    return float(lr)
+
+
+def _momentum_table(op, vars_, accums, grads):
+    """The device table of d3f_momentum_clip_update: int64 [T, 4] = (var, accum, grad, numel), copied from pinned
+    memory without a synchronisation. vars_ and accums are updated in place (contiguous, or ValueError); a strided
+    grad is read through a contiguous copy. The returned list keeps every tensor the table names alive, so none of its
+    addresses can be freed and handed to another tensor while the table is in use. Refused (RuntimeError) while the
+    current stream is being captured into a CUDA graph: the graph would copy from a pinned buffer that does not outlive
+    the capture."""
+    dev, rows, keep = None, [], []
+    for i, (v, a, g) in enumerate(zip(vars_, accums, grads)):
+        for t, n in ((v, "var"), (a, "accum")):
+            if not (torch.is_tensor(t) and t.is_contiguous()):
+                raise ValueError("%s: %s[%d] must be a contiguous tensor (it is updated in place)" % (op, n, i))
+        v = _lib.tensor_arg(v, "%s: var[%d]" % (op, i), _F32, None, dev)
+        dev = v.device
+        a = _lib.tensor_arg(a, "%s: accum[%d]" % (op, i), _F32, tuple(v.shape), dev)
+        g = _lib.tensor_arg(g, "%s: grad[%d]" % (op, i), _F32, tuple(v.shape), dev)
+        keep += [v, a, g]
+        rows.append((v.data_ptr(), a.data_ptr(), g.data_ptr(), v.numel()))
+    if torch.cuda.is_current_stream_capturing():
+        raise RuntimeError("%s: the table of tensor addresses cannot be built during CUDA graph capture; run one eager "
+                           "step with the same tensors before capturing" % op)
+    host = torch.tensor(rows, dtype=torch.int64).reshape(-1, 4).pin_memory()
+    return host.to(dev, non_blocking=True), keep, sum(r[3] for r in rows)
+
+
+def _momentum_launch(op, table, T, numel, lr, momentum, clip_norm, dev):
+    L = _lib.lib()
+    ws = _lib.workspace(L.d3f_momentum_clip_workspace_bytes(T, numel), dev)
+    _lib.check(L.d3f_momentum_clip_update(_lib.ptr(table), T, numel, float(np.float32(lr)),
+                                          float(np.float32(momentum)), float(np.float32(clip_norm)), _lib.ptr(ws),
+                                          ws.numel(), _lib.stream()), op)
+
+
+def momentum_clip_update(vars_, accums, grads, lr, momentum, clip_norm):
+    """One update of the reference's trainer for every tensor of the lists, in place (utils/trainer.py:116-156):
+    gc = tf.clip_by_norm(g, clip_norm) (none for clip_norm <= 0), accum = accum * momentum + gc, var -= accum * lr.
+    The exact contract, with the fp64 block-ordered norm, is oracle/optim_np.py. Two kernels for all tensors, no
+    synchronisation. It copies a fresh table of addresses every call, so it cannot be captured in a CUDA graph; a
+    MomentumClip step can."""
+    op = "momentum_clip_update"
+    vars_, accums, grads = list(vars_), list(accums), list(grads)
+    if not len(vars_) == len(accums) == len(grads):
+        raise ValueError("%s: %d vars, %d accums and %d grads" % (op, len(vars_), len(accums), len(grads)))
+    if not vars_:
+        return
+    table, keep, numel = _momentum_table(op, vars_, accums, grads)
+    _momentum_launch("d3f_momentum_clip_update", table, len(vars_), numel, lr, momentum, clip_norm, table.device)
+    for v in vars_:
+        torch.autograd.graph.increment_version(v)
+
+
+class MomentumClip:
+    """The reference's update: tf.clip_by_norm on each gradient on its own, then tf.train.MomentumOptimizer
+    (utils/trainer.py:116-156), as two sm_90a kernels for all parameters together (d3f_momentum_clip_update). It
+    differs from torch.optim.SGD + clip_grad_norm_: torch adds 1e-6 to the norm and leaves g alone below the threshold,
+    where TF always computes g * c / max(norm, c), which can move g by an ulp; and SGD's momentum applies lr to the
+    gradient before the accumulator, not after. The norm is summed in fp64 in fixed blocks (oracle/optim_np.py), so
+    every step is bitwise reproducible.
+
+    params: float32 contiguous CUDA tensors on one device (updated in place). state: the accumulators (TF's Momentum
+    slots), zero-initialised, one per parameter. lr, momentum, clip_norm are read at every step() (clip_norm <= 0: no
+    clipping), rounded to float32. A parameter whose .grad is None is skipped, as TF skips a None gradient. An entry of
+    state (or the whole list) may be replaced, e.g. by restored slots, and a parameter's storage may be replaced
+    (p.data = ...): the next step() uses the new tensors.
+
+    step() never synchronises. It keeps a device table of the parameters', accumulators' and gradients' addresses and
+    rebuilds it (one pinned copy) only when one of them moves or changes size; zero_grad() zeroes the gradients in
+    place, so the addresses stay. To capture step() in a CUDA graph, run one eager step() with the same tensors first:
+    a step that would rebuild the table during the capture raises RuntimeError. The graph then replays on those
+    tensors, with the lr, momentum and clip_norm of the capture."""
+
+    def __init__(self, params, lr, momentum, clip_norm):
+        self.params = list(params)
+        dev = None
+        for i, p in enumerate(self.params):
+            if not (torch.is_tensor(p) and p.is_contiguous()):
+                raise ValueError("MomentumClip: params[%d] must be a contiguous tensor (it is updated in place)" % i)
+            dev = _lib.tensor_arg(p, "MomentumClip: params[%d]" % i, _F32, None, dev).device
+        self.lr, self.momentum, self.clip_norm = float(lr), float(momentum), float(clip_norm)
+        self.state = [torch.zeros_like(p, memory_format=torch.contiguous_format) for p in self.params]
+        self._key, self._table = None, None
+
+    def zero_grad(self):
+        """Zero every existing gradient in place (addresses kept)."""
+        with torch.no_grad():
+            for p in self.params:
+                if p.grad is not None:
+                    p.grad.zero_()
+
+    def step(self):
+        live = [i for i, p in enumerate(self.params) if p.grad is not None]
+        if not live:
+            return
+        if len(self.state) != len(self.params):
+            raise ValueError("MomentumClip.step: %d accumulators in state for %d parameters" % (
+                len(self.state), len(self.params)))
+        triples = [(self.params[i].detach(), self.state[i], self.params[i].grad) for i in live]
+        # every address and size the kernel reads or writes through: a moved parameter, accumulator or gradient
+        # rebuilds the table
+        key = tuple((i,) + tuple((t.data_ptr(), t.numel(), t.is_contiguous()) if torch.is_tensor(t) else (id(t),)
+                                 for t in ts) for i, ts in zip(live, triples))
+        if key != self._key or not all(g.is_contiguous() for _, _, g in triples):
+            self._table = _momentum_table("MomentumClip.step", *zip(*triples))
+            self._key = key
+        table, _, numel = self._table
+        _momentum_launch("d3f_momentum_clip_update", table, len(live), numel, self.lr, self.momentum, self.clip_norm,
+                         table.device)
+        for i in live:
+            torch.autograd.graph.increment_version(self.params[i])

@@ -45,6 +45,9 @@
  *   d3f_evaluate_pairs        geometric_registration/evaluate.py:67-82,207, repeatability/evaluate_3dmatch_our.py:30-41,
  *                             evaluate_kitti_our.py:12-23, utils/tester.py:326-342, 3dmatch/evaluate.m with
  *                             mrEvaluateRegistration.m (FMR, repeatability, RTE / RRE, registration recall)
+ *   d3f_momentum_clip_update  utils/trainer.py:116-156 (tf.clip_by_norm per gradient + tf.train.MomentumOptimizer)
+ *   d3f_rank_mean             the data-parallel mean of gradients and batch statistics over ranks (no counterpart:
+ *                             the reference trains on one GPU)
  */
 #ifndef D3FEAT_B200_H_
 #define D3FEAT_B200_H_
@@ -617,6 +620,40 @@ int d3f_augment_pairs(const float* points, const int* lengths, int B, int N, con
                       double scale_min, double scale_max, double shift_range, int capacity, float* out_points,
                       float* backup_points, int* out_lengths, long long* row_offset, float* R, double* scale,
                       double* shift, void* workspace, size_t workspace_bytes, d3f_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * The training update (utils/trainer.py:116-156): tf.clip_by_norm on each gradient on its own (TF 1.12
+ * clip_ops.clip_by_norm), then tf.train.MomentumOptimizer (ApplyMomentum, use_nesterov = False). Contract:
+ * oracle/optim_np.py, exactly. table[T] (device) names T tensors; per tensor, in fp32 with one rounding per operation
+ * and no fused multiply-add:
+ *   l2sum = sum of g^2 in fp64: each 2048-element block (from element 0) summed sequentially, the blocks added in
+ *           block order. TF sums g*g in fp32 in an unspecified order: the one deviation.
+ *   norm  = fl32(sqrt(l2sum)), 0 when l2sum = 0 (TF's where(l2sum > 0, ...)); M = (norm < c) ? c : norm
+ *   gc    = fl32(fl32(g * c) / M)          (clip_norm = c <= 0: gc = g, trainer.py:150-153, and no norm is taken)
+ *   accum = fl32(fl32(accum * momentum) + gc);   var = fl32(var - fl32(accum * lr))
+ * Two kernels for all tensors together (one without clipping): block partials over the flat element space, then
+ * per-tensor finalise and update. No float atomics, no host synchronisation: graph-capturable, bitwise identical run to
+ * run and across streams. numel_total (host) must equal the sum of the table's numel: the workspace is sized from it
+ * (d3f_momentum_clip_workspace_bytes(T, numel_total)); any other table gives an unspecified update but never writes
+ * outside the workspace or the named tensors. A numel < 0 counts as 0. T in [0, 1024], numel_total >= 0; var, accum
+ * and grad of one tensor must not overlap. Otherwise, or for a null pointer, D3F_ERR_INVALID before any CUDA call.
+ *
+ * d3f_rank_mean: the data-parallel reduction of a gathered x[R, P] (device, fp32, rank-major):
+ *   out[p] = fl32((x[0,p] + x[1,p] + ... + x[R-1,p]) / R), summed in fp64 in rank order from x[0,p]
+ * (R = 1: out = x bit for bit; for R > 1 a NaN comes out as the canonical NaN). out may be x's row 0. R >= 1,
+ * P >= 0. One kernel (none for P = 0).
+ * ------------------------------------------------------------------------------------------- */
+typedef struct {
+  float* var;
+  float* accum;
+  const float* grad;
+  long long numel;
+} d3f_momentum_tensor;
+size_t d3f_momentum_clip_workspace_bytes(int T, long long numel_total);
+int d3f_momentum_clip_update(const d3f_momentum_tensor* table, int T, long long numel_total, float lr,
+                             float momentum, float clip_norm, void* workspace, size_t workspace_bytes,
+                             d3f_stream_t stream);
+int d3f_rank_mean(const float* x, int R, long long P, float* out, d3f_stream_t stream);
 
 #ifdef __cplusplus
 }
