@@ -10,13 +10,16 @@ Same function names and signatures as the reference so that architecture lists a
                                                                        424-471, 561-612, 672-723, 971-979
   get_block_ops(block_name)                       :982-1042
   assemble_CNN_blocks(inputs, config, dropout_prob)   :1052-1118  (the ENCODER)
+  assemble_FCNN_blocks / assemble_FCNN_decoder    models/D3Feat.py:5-115
 
-Inference only (training = dropout_prob < 0.99 must be False, like utils/tester.py:199 feeds 1.0): batch
-norm uses the moving statistics and is folded, together with the LeakyReLU and the residual add, into the
+The blocks are inference only (training = dropout_prob < 0.99 must be False, like utils/tester.py:199 feeds 1.0):
+batch norm uses the moving statistics and is folded, together with the LeakyReLU and the residual add, into the
 epilogue of the producing kernel. Parameters are looked up in the active ParamStore under the reference's
-variable-scope names.
+variable-scope names. The schedule of scopes, radii and widths (architecture, run_blocks) is shared with the training
+blocks (training.forward) and the seeded parameters (synth.make_params).
 """
-import numpy as np
+from collections import namedtuple
+
 import torch
 
 from . import _lib
@@ -100,28 +103,26 @@ def _affine_leaky(x, scale, shift, residual, alpha, rows=None):
     return out
 
 
+def _bn_affine(use_batch_norm):
+    """(scale, shift) of the current scope's inference batch norm (:149-160), or scale 1 and the 'offset' bias without
+    batch norm (:162-165)."""
+    store, scope = V.current_store(), V.current_scope()
+    if use_batch_norm:
+        return store.bn_affine(scope)
+    shift = store.bn_variables(scope, False)[1]
+    return torch.ones_like(shift), shift
+
+
 def _bn_epilogue(config, alpha):
-    """(scale, shift, alpha) of the current scope's inference batch norm (:149-160)."""
-    store = V.current_store()
-    if config.use_batch_norm:
-        scale, shift = store.bn_affine(V.current_scope())
-    else:                                            # 'offset' bias only (:162-165)
-        shift = store.get(V.scoped("offset"))
-        scale = torch.ones_like(shift)
-    return scale, shift, alpha
+    """(scale, shift, alpha): the current scope's batch norm and LeakyReLU as a kernel epilogue."""
+    return _bn_affine(config.use_batch_norm) + (alpha,)
 
 
 def batch_norm(x, use_batch_norm=True, momentum=0.99, training=True):
     """:149-165, inference form only (moving statistics, epsilon 1e-6)."""
     if training:
         raise NotImplementedError("d3feat_b200 implements the inference path (training = dropout_prob < 0.99 is False)")
-    store = V.current_store()
-    if use_batch_norm:
-        scale, shift = store.bn_affine(V.current_scope())
-    else:
-        shift = store.get(V.scoped("offset"))
-        scale = torch.ones_like(shift)
-    return _affine_leaky(x, scale, shift, None, None)
+    return _affine_leaky(x, *_bn_affine(use_batch_norm), None, None)
 
 
 def leaky_relu(features, alpha=0.2):
@@ -272,35 +273,59 @@ def get_block_ops(block_name):
 #  architectures
 # ----------------------------------------------------------------------------------------------------
 
+# One block of the schedule: its name, pyramid layer, variable scope, radius and width (fdim). skip: the running
+# features join the skip list F before the block; concat: F[layer - 1] is concatenated to the block's output.
+Step = namedtuple("Step", "block layer scope radius fdim skip concat")
+
+
+def architecture(config):
+    """The schedule of config.architecture as (encoder, decoder), two lists of Steps: the walk of assemble_CNN_blocks
+    (models/network_blocks.py:1052-1118) and of the decoder loop of models/D3Feat.py:15-63, which starts at the first
+    upsample block (no decoder without one). Scopes are 'layer_{l}/{block}_{i}' without '_deformable' and
+    'uplayer_{l}/{block}_{i}'. Radius (from first_subsampling_dl * density_parameter) and fdim (from first_features_dim)
+    double after every pool / strided block; the decoder starts them at the deepest layer and halves them after every
+    upsample block. The inference blocks, training.forward and synth.make_params all walk this one schedule."""
+    arch = list(config.architecture)
+    start = next((i for i, b in enumerate(arch) if "upsample" in b), len(arch))
+    r0, f0 = config.first_subsampling_dl * config.density_parameter, config.first_features_dim
+    encoder, decoder = [], []
+    layer, r, fdim, i = 0, r0, f0, 0
+    for block in arch[:start]:
+        down = "pool" in block or "strided" in block
+        scope = "layer_{:d}/{:s}_{:d}".format(layer, block.replace("_deformable", ""), i)
+        encoder.append(Step(block, layer, scope, r, fdim, down or "global" in block, False))
+        layer, r, fdim, i = (layer + 1, r * 2, fdim * 2, 0) if down else (layer, r, fdim, i + 1)
+    layer = config.num_layers - 1
+    r, fdim, i = r0 * 2 ** layer, f0 * 2 ** layer, 0
+    for block in arch[start:]:
+        up = "upsample" in block
+        decoder.append(Step(block, layer, "uplayer_{:d}/{:s}_{:d}".format(layer, block, i), r, fdim, False, up))
+        layer, r, fdim, i = (layer - 1, r * 0.5, fdim // 2, 0) if up else (layer, r, fdim, i + 1)
+    return encoder, decoder
+
+
+def run_blocks(steps, block_ops, inputs, features, F, config, *args):
+    """Run `steps` of architecture(config) on `features`, each under its variable scope, as
+    block_ops(step.block)(layer, inputs, features, radius, fdim, config, *args). The running features are appended to
+    F before a step with .skip; F[layer - 1] is concatenated to the output of one with .concat. Returns the last
+    features."""
+    for s in steps:
+        if s.skip:
+            F.append(features)
+        with variable_scope(s.scope):
+            features = block_ops(s.block)(s.layer, inputs, features, s.radius, s.fdim, config, *args)
+        if s.concat:
+            features = torch.cat((features, F[s.layer - 1]), dim=1)
+    return features
+
+
 def assemble_CNN_blocks(inputs, config, dropout_prob):
-    """:1052-1118 -- the KPFCNN encoder. Returns F, the list of per-level skip features (and, for an
-    encoder-only architecture without upsample blocks, the final features as the last entry)."""
-    r = config.first_subsampling_dl * config.density_parameter
-    layer = 0
-    fdim = config.first_features_dim
-    features = inputs["features"]
+    """:1052-1118 -- the KPFCNN encoder. Returns F, the list of per-level skip features with the final features as
+    the last entry."""
     F = []
-    training = dropout_prob < 0.99
-    block_in_layer = 0
-    saw_upsample = False
-    for block_i, block in enumerate(config.architecture):
-        if np.any([tmp in block for tmp in ["pool", "strided", "upsample", "global"]]):
-            F += [features]
-        if "upsample" in block:
-            saw_upsample = True
-            break
-        with variable_scope("layer_{:d}/{:s}_{:d}".format(layer, block.replace("_deformable", ""), block_in_layer)):
-            block_ops = get_block_ops(block)
-            features = block_ops(layer, inputs, features, r, fdim, config, training)
-        block_in_layer += 1
-        if "pool" in block or "strided" in block:
-            layer += 1
-            r *= 2
-            fdim *= 2
-            block_in_layer = 0
-    if not saw_upsample:
-        F += [features]
-    return F
+    features = run_blocks(architecture(config)[0], get_block_ops, inputs, inputs["features"], F, config,
+                          dropout_prob < 0.99)
+    return F + [features]
 
 
 def detection_scores(features, neighbors, lengths, *, rows=None):
@@ -341,29 +366,11 @@ def assemble_FCNN_blocks(inputs, config, dropout_prob=1.0):
 
 def assemble_FCNN_decoder(inputs, config, F, dropout_prob=1.0, with_scores=False):
     """models/D3Feat.py:15-65 -- decoder loop + l2-normalised 32-d descriptors; with_scores=True also runs the
-    detection branch (:67-115) and returns (descriptors, scores)."""
-    features = F[-1]
-    layer = config.num_layers - 1
-    r = config.first_subsampling_dl * config.density_parameter * 2 ** layer
-    fdim = config.first_features_dim * 2 ** layer
-    training = dropout_prob < 0.99
-    start_i = 0
-    for block_i, block in enumerate(config.architecture):
-        if "upsample" in block:
-            start_i = block_i
-            break
-    block_in_layer = 0
-    for block_i, block in enumerate(config.architecture[start_i:]):
-        with variable_scope("uplayer_{:d}/{:s}_{:d}".format(layer, block, block_in_layer)):
-            block_ops = get_block_ops(block)
-            features = block_ops(layer, inputs, features, r, fdim, config, training)
-        block_in_layer += 1
-        if "upsample" in block:
-            layer -= 1
-            r *= 0.5
-            fdim = fdim // 2
-            block_in_layer = 0
-            features = torch.cat((features, F[layer]), dim=1)
+    detection branch (:67-115) and returns (descriptors, scores). ValueError for an architecture without a decoder."""
+    decoder = architecture(config)[1]
+    if not decoder:
+        raise ValueError("assemble_FCNN_decoder: the architecture has no upsample block, so no decoder")
+    features = run_blocks(decoder, get_block_ops, inputs, F[-1], F, config, dropout_prob < 0.99)
     out = l2_normalize(features, rows=_rows(inputs, 0))
     if with_scores:
         return out, detection_scores(features, inputs["neighbors"][0], inputs["lengths"][0], rows=_rows(inputs, 0))

@@ -17,6 +17,9 @@ rounded to 1e-3) under the reference's variable names.
 """
 import numpy as np
 
+from .network_blocks import architecture
+from .variables import ParamStore
+
 ARCH_3DMATCH = ["simple", "resnetb",
                 "resnetb_strided", "resnetb",
                 "resnetb_strided", "resnetb",
@@ -234,33 +237,24 @@ def _bn(rng, params, scope, dim, trained_like):
         v = rng.uniform(0.5, 1.5, dim)
     else:
         g, b, m, v = np.ones(dim), np.zeros(dim), np.zeros(dim), np.ones(dim)
-    pre = scope + "/batch_normalization/"
-    params[pre + "gamma"] = g.astype(np.float32)
-    params[pre + "beta"] = b.astype(np.float32)
-    params[pre + "moving_mean"] = m.astype(np.float32)
-    params[pre + "moving_variance"] = v.astype(np.float32)
+    for name, x in zip(ParamStore.bn_names(scope), (g, b, m, v)):
+        params[name] = x.astype(np.float32)
 
 
 def make_params(config, seed=0, trained_like_bn=True):
-    """Seeded weights / BN statistics / kernel points under the reference's variable scopes
-    (models/network_blocks.py:1087 'layer_{l}/{block}_{i}', models/D3Feat.py:37 'uplayer_...')."""
+    """Seeded weights / BN statistics / kernel points under the reference's variable scopes, walked by
+    network_blocks.architecture ('layer_{l}/{block}_{i}', 'uplayer_{l}/{block}_{i}')."""
     rng = np.random.default_rng(seed)
     p = {}
     K = config.num_kernel_points
-    r = config.first_subsampling_dl * config.density_parameter
-    layer, fdim, bil = 0, config.first_features_dim, 0
     cin = config.in_features_dim
     skip_dims = []
-    arch = list(config.architecture)
-    i = 0
-    while i < len(arch):
-        block = arch[i]
-        if "upsample" in block:
-            break
-        if "pool" in block or "strided" in block:
+    encoder, decoder = architecture(config)
+    for step in encoder:
+        block, scope, fdim = step.block, step.scope, step.fdim
+        if step.skip:
             skip_dims.append(cin)
-        scope = "layer_{:d}/{:s}_{:d}".format(layer, block.replace("_deformable", ""), bil)
-        extent = config.KP_extent * r / config.density_parameter
+        extent = config.KP_extent * step.radius / config.density_parameter
         if block == "simple":
             p[scope + "/weights"] = weight_variable(rng, (K, cin, fdim))
             p[scope + "/kernel_points"] = kernel_points(rng, 1.5 * extent, K)
@@ -287,32 +281,14 @@ def make_params(config, seed=0, trained_like_bn=True):
             cin = 2 * fdim
         else:
             raise ValueError("Unknown block name in the architecture definition : " + block)
-        bil += 1
-        if "pool" in block or "strided" in block:
-            layer += 1
-            r *= 2
-            fdim *= 2
-            bil = 0
-        i += 1
-    # decoder (models/D3Feat.py:15-63)
-    if i < len(arch):
-        skip_dims.append(cin)
-        layer = config.num_layers - 1
-        fdim = config.first_features_dim * 2 ** layer
-        bil = 0
-        for block in arch[i:]:
-            scope = "uplayer_{:d}/{:s}_{:d}".format(layer, block, bil)
-            if block == "unary":
-                p[scope + "/weights"] = weight_variable(rng, (cin, fdim))
-                _bn(rng, p, scope, fdim, trained_like_bn)
-                cin = fdim
-            elif block == "last_unary":
-                p[scope + "/weights"] = weight_variable(rng, (cin, 32))
-                cin = 32
-            bil += 1
-            if "upsample" in block:
-                layer -= 1
-                fdim //= 2
-                bil = 0
-                cin = cin + skip_dims[layer]
+    for step in decoder:
+        if step.block == "unary":
+            p[step.scope + "/weights"] = weight_variable(rng, (cin, step.fdim))
+            _bn(rng, p, step.scope, step.fdim, trained_like_bn)
+            cin = step.fdim
+        elif step.block == "last_unary":
+            p[step.scope + "/weights"] = weight_variable(rng, (cin, 32))
+            cin = 32
+        if step.concat:
+            cin += skip_dims[step.layer - 1]
     return p

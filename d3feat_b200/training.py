@@ -13,10 +13,10 @@ models/D3Feat.py with training = True, and the loss of models/KPFCNN_model.py:14
 The differentiable ops are torch.autograd.Functions over sm_90a kernels (train_ops.cu): batch norm in training mode
 (batch statistics, moving-average update in place), ind_max_pool, closest_pool / gather_rows, l2_normalize and
 detection_scores. The update is MomentumClip over optim.cu. The convolutions are the differentiable conv_ops.KPConv /
-unary_convolution. The inference path (network_blocks, encoder.KPFCNN) is untouched and still refuses
-training = True; because the moving statistics are updated in place, ParamStore.bn_affine picks the trained
-statistics up. The loss is small tensor algebra on the
-keypoints and stays in torch.
+unary_convolution. forward walks the same schedule of scopes, radii and widths as the inference path
+(network_blocks.architecture), with its own blocks; the inference blocks still refuse training = True. Because the
+moving statistics are updated in place, ParamStore.bn_affine picks the trained statistics up. The loss is small tensor
+algebra on the keypoints and stays in torch.
 
 The step is not graph-capturable (the KPConv feature gradient reads its reverse width back to the host), so inputs
 must have exact shapes: a static (capacity-sized) pyramid is refused with ValueError. Deformable blocks have no
@@ -267,12 +267,7 @@ def batch_norm(x, scope, config, residual=None, alpha=None):
     store = V.current_store()
     if store is None:
         raise RuntimeError("batch_norm: no ParamStore active (wrap the call in variables.use_params)")
-    if config.use_batch_norm:
-        pre = scope + "/batch_normalization/"
-        gamma, beta = store.get(pre + "gamma"), store.get(pre + "beta")
-        mm, mv = store.get(pre + "moving_mean"), store.get(pre + "moving_variance")
-    else:
-        gamma, beta, mm, mv = None, store.get(scope + "/offset"), None, None
+    gamma, beta, mm, mv = store.bn_variables(scope, config.use_batch_norm)
     return _BatchNormFn.apply(x, gamma, beta, residual, mm, mv, float(config.batch_norm_momentum), alpha)
 
 
@@ -386,66 +381,23 @@ def get_block_ops(block_name):
     return BLOCKS[block_name]
 
 
-def check_inputs(inputs, config):
-    """ValueError for a static (capacity-sized) pyramid; NotImplementedError for a deformable architecture. Both
-    before anything runs."""
+def forward(inputs, config):
+    """assemble_FCNN_blocks (models/D3Feat.py:5-115) with training = True, under the active ParamStore: the schedule
+    of network_blocks.architecture run with the blocks above -> (l2-normalised descriptors [N, 32], scores [N, 1]).
+    Updates the moving statistics of every batch norm in place. Before anything runs: ValueError for a static
+    (capacity-sized) pyramid or an architecture without a decoder, NotImplementedError for a deformable one."""
     if inputs.get("rows"):
         raise ValueError("training: the inputs are a static (capacity-sized) pyramid; training needs exact shapes "
                          "(pyramid.descriptor_input without static=True)")
     for block in config.architecture:
         get_block_ops(block)
-
-
-def encoder(inputs, config):
-    """assemble_CNN_blocks (models/network_blocks.py:1052-1118) with training = True -> skip features F."""
-    r = config.first_subsampling_dl * config.density_parameter
-    layer, fdim, block_in_layer = 0, config.first_features_dim, 0
-    features = inputs["features"]
+    encoder, decoder = nb.architecture(config)
+    if not decoder:
+        raise ValueError("training: the architecture has no upsample block, so no decoder")
     F = []
-    for block in config.architecture:
-        if any(t in block for t in ("pool", "strided", "upsample", "global")):
-            F.append(features)
-        if "upsample" in block:
-            break
-        with variable_scope("layer_{:d}/{:s}_{:d}".format(layer, block.replace("_deformable", ""), block_in_layer)):
-            features = get_block_ops(block)(layer, inputs, features, r, fdim, config)
-        block_in_layer += 1
-        if "pool" in block or "strided" in block:
-            layer += 1
-            r *= 2
-            fdim *= 2
-            block_in_layer = 0
-    if not any("upsample" in b for b in config.architecture):
-        F.append(features)
-    return F
-
-
-def decoder(inputs, config, F):
-    """models/D3Feat.py:15-115 with training = True -> (l2-normalised descriptors [N, 32], scores [N, 1])."""
-    features = F[-1]
-    layer = config.num_layers - 1
-    r = config.first_subsampling_dl * config.density_parameter * 2 ** layer
-    fdim = config.first_features_dim * 2 ** layer
-    start = next(i for i, b in enumerate(config.architecture) if "upsample" in b)
-    block_in_layer = 0
-    for block in config.architecture[start:]:
-        with variable_scope("uplayer_{:d}/{:s}_{:d}".format(layer, block, block_in_layer)):
-            features = get_block_ops(block)(layer, inputs, features, r, fdim, config)
-        block_in_layer += 1
-        if "upsample" in block:
-            layer -= 1
-            r *= 0.5
-            fdim = fdim // 2
-            block_in_layer = 0
-            features = torch.cat((features, F[layer]), dim=1)
+    features = nb.run_blocks(encoder, get_block_ops, inputs, inputs["features"], F, config)
+    features = nb.run_blocks(decoder, get_block_ops, inputs, features, F, config)
     return l2_normalize(features), detection_scores(features, inputs["neighbors"][0], inputs["lengths"][0])
-
-
-def forward(inputs, config):
-    """assemble_FCNN_blocks with training = True, under the active ParamStore: (descriptors, scores). Updates the
-    moving statistics of every batch norm in place."""
-    check_inputs(inputs, config)
-    return decoder(inputs, config, encoder(inputs, config))
 
 
 def trainable(store):

@@ -45,12 +45,24 @@ class ParamStore:
         except KeyError:
             raise KeyError("variable '%s' is not in the parameter store" % name)
 
+    @staticmethod
+    def bn_names(scope):
+        """The variables tf.layers.batch_normalization creates under `scope` (models/network_blocks.py:149-160):
+        '<scope>/batch_normalization/' + gamma, beta, moving_mean, moving_variance."""
+        return tuple(scope + "/batch_normalization/" + k for k in ("gamma", "beta", "moving_mean", "moving_variance"))
+
+    def bn_variables(self, scope, use_batch_norm=True):
+        """(gamma, beta, moving_mean, moving_variance) of `scope`'s batch norm; with use_batch_norm off,
+        (None, offset, None, None): the '<scope>/offset' bias that replaces it (models/network_blocks.py:162-165)."""
+        if use_batch_norm:
+            return tuple(self.get(n) for n in self.bn_names(scope))
+        return None, self.get(scope + "/offset"), None, None
+
     def bn_affine(self, scope, eps=1e-6):
         """Inference batch norm folded to y = x*scale + shift (models/network_blocks.py:149-160 with moving
         statistics): scale = gamma / sqrt(var + eps), shift = beta - mean * scale. Folded in float64, once per
         scope, and again when one of the four tensors is replaced or updated in place."""
-        pre = scope + "/batch_normalization/"
-        src = tuple(self.t[pre + k] for k in ("gamma", "beta", "moving_mean", "moving_variance"))
+        src = self.bn_variables(scope)
         key = (scope, eps)
         hit = self._bn.get(key)
         if hit is not None and all(a is b and a._version == v for a, b, v in zip(src, hit[0], hit[1])):
