@@ -2,6 +2,8 @@
 clouds, and the per-fragment arrays the reference's offline evaluation consumes.
 
   * load_config      -- utils/config.py:Config.load (parameters.txt -> attributes; only the keys the path reads)
+  * save_config      -- utils/config.py:Config.save for those keys and the trainer's schedule (trainer.Trainer)
+  * write_ply_points -- utils/ply.py:write_ply of x/y/z (the trainer's kernel_points/epoch*/ files)
   * read_ply_points  -- utils/ply.py:read_ply, vertex x/y/z of ascii / binary PLY files
   * select_keypoints -- utils/tester.py:209-213 (3DMatch: all points, ascending score) and :283-290 (KITTI: top-k)
   * write_fragment   -- utils/tester.py:226-228: descriptors/<scene>/cloud_bin_N.D3Feat.npy,
@@ -47,6 +49,60 @@ def load_config(path):
         if k in kw:
             kw[k] = bool(kw[k])
     return Config(**kw)
+
+
+def save_config(config, path, dataset=None):
+    """utils/config.py:Config.save for the keys load_config reads (and the trainer's own: the learning-rate schedule,
+    max_epoch, epoch_steps, validation_size, snapshot_gap) in the reference's line formats and section layout: writes
+    path/parameters.txt. A key the config does not have is left out; dataset fills in a config without one."""
+    def has(k):
+        return getattr(config, k, None) is not None
+
+    lines = ["# -----------------------------------#", "# Parameters of the training session #",
+             "# -----------------------------------#", "", "# Input parameters", "# ****************", ""]
+    fmt = dict(in_points_dim="{:d}", in_features_dim="{:d}", in_radius="{:.3f}", input_threads="{:d}",
+               num_layers="{:d}", first_features_dim="{:d}", use_batch_norm="{:d}", batch_norm_momentum="{:.3f}",
+               first_subsampling_dl="{:.3f}", num_kernel_points="{:d}", density_parameter="{:.3f}",
+               fixed_kernel_points="{:s}", KP_extent="{:.3f}", KP_influence="{:s}", convolution_mode="{:s}",
+               modulated="{:d}", learning_rate="{:f}", momentum="{:f}", grad_clip_norm="{:f}", weights_decay="{:f}",
+               batch_num="{:d}", max_epoch="{:d}", epoch_steps="{:d}", validation_size="{:d}", snapshot_gap="{:d}")
+
+    def put(*keys):
+        for k in keys:
+            if has(k):
+                v = getattr(config, k)
+                lines.append((k + " = " + fmt[k]).format(int(v) if fmt[k] == "{:d}" else v))
+
+    name = getattr(config, "dataset", None) or dataset
+    if name is not None:
+        lines.append("dataset = {:s}".format(name))
+    put("in_points_dim", "in_features_dim", "in_radius", "input_threads")
+    lines += ["", "# Model parameters", "# ****************", "",
+              "architecture =" + "".join(" {:s}".format(a) for a in config.architecture)]
+    put("num_layers", "first_features_dim", "use_batch_norm", "batch_norm_momentum")
+    lines += ["", "# KPConv parameters", "# *****************", ""]
+    put("first_subsampling_dl", "num_kernel_points", "density_parameter", "fixed_kernel_points", "KP_extent",
+        "KP_influence", "convolution_mode", "modulated")
+    lines += ["", "# Training parameters", "# *******************", ""]
+    put("learning_rate", "momentum")
+    if getattr(config, "lr_decays", None):
+        lines.append("lr_decay_epochs =" + "".join(" {:d}:{:f}".format(e, d) for e, d in config.lr_decays.items()))
+    put("grad_clip_norm", "weights_decay", "batch_num", "max_epoch", "epoch_steps", "validation_size", "snapshot_gap")
+    os.makedirs(path, exist_ok=True)
+    out = os.path.join(path, "parameters.txt")
+    with open(out, "w") as fh:
+        fh.write("\n".join(lines) + "\n")
+    return out
+
+
+def write_ply_points(path, points):
+    """float32 [N,3] points as a binary little-endian PLY with vertex x/y/z (utils/ply.py:write_ply's layout)."""
+    pts = np.ascontiguousarray(points, np.float32).reshape(-1, 3)
+    head = "ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\n" \
+           "property float z\nend_header\n" % pts.shape[0]
+    with open(path, "wb") as fh:
+        fh.write(head.encode("ascii"))
+        fh.write(pts.astype("<f4").tobytes())
 
 
 _PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2", "ushort": "u2",

@@ -53,11 +53,44 @@ def _make_crc_table():
 _CRC_TABLE = _make_crc_table()
 
 
+_CHUNK = 4096
+_SHIFT = []                                 # byte tables of "feed _CHUNK zero bytes", built on first use
+
+
+def _shift_tables():
+    """T[i][v]: the register after _CHUNK zero bytes from register v << 8i. The map is linear over GF(2), so the
+    register r goes to T[0][r & 255] ^ T[1][r >> 8 & 255] ^ T[2][r >> 16 & 255] ^ T[3][r >> 24]."""
+    if not _SHIFT:
+        r = (np.arange(256, dtype=np.uint32)[None, :] << (8 * np.arange(4, dtype=np.uint32))[:, None]).reshape(-1)
+        for _ in range(_CHUNK):
+            r = _CRC_TABLE[r & 0xFF] ^ (r >> 8)
+        _SHIFT.extend(int(x) for x in r)
+    return _SHIFT
+
+
+def _crc_register_chunked(c, data):
+    """The register after `data` (a multiple of _CHUNK bytes) from register c: every chunk's register from 0 at once
+    (one table step per byte position, across all chunks), then chained: r = shift(r) ^ chunk register."""
+    rows = np.frombuffer(data, np.uint8).reshape(-1, _CHUNK)
+    z = np.zeros(rows.shape[0], np.uint32)
+    for j in range(_CHUNK):
+        z = _CRC_TABLE[(z ^ rows[:, j]) & 0xFF] ^ (z >> 8)
+    T = _shift_tables()
+    for v in z.tolist():
+        c = T[c & 0xFF] ^ T[256 + (c >> 8 & 0xFF)] ^ T[512 + (c >> 16 & 0xFF)] ^ T[768 + (c >> 24)] ^ v
+    return c
+
+
 def crc32c(data, crc=0):
-    """Castagnoli CRC. Byte-serial (table driven): meant for index blocks and small tensors."""
+    """Castagnoli CRC. Table driven, byte-serial below 64 KiB; longer inputs go through _CHUNK-byte chunks whose
+    registers are computed side by side in numpy and then chained (the same value, at numpy speed)."""
     tab = _CRC_TABLE
     c = (~crc) & 0xFFFFFFFF
-    for b in bytes(data):
+    data = bytes(data)
+    head = len(data) - len(data) % _CHUNK if len(data) >= 1 << 16 else 0
+    if head:
+        c = _crc_register_chunked(c, data[:head])
+    for b in data[head:]:
         c = int(tab[(c ^ b) & 0xFF]) ^ (c >> 8)
     return (~c) & 0xFFFFFFFF
 
@@ -337,3 +370,30 @@ def write_checkpoint(prefix, tensors, block_entries=64):
         index_handle = _emit_block(fh, _block(index, restart_interval=1))
         foot = meta_handle + index_handle
         fh.write(foot + b"\x00" * (40 - len(foot)) + struct.pack("<Q", _MAGIC))
+
+
+# ---------------------------------------------------------------------------------------------------- optimizer slots
+
+MOMENTUM_SLOT = "/Momentum"                 # tf.train.MomentumOptimizer's slot: '<variable>/Momentum'
+
+
+def write_slots(prefix, slots, extra=None):
+    """Writes the momentum accumulators {store name: ndarray} as a bundle, each under MODEL_SCOPE + name + '/Momentum'
+    (the name TF gives the slot), plus the `extra` {name: ndarray} entries as they are (names outside MODEL_SCOPE)."""
+    tensors = {MODEL_SCOPE + n + MOMENTUM_SLOT: np.asarray(a) for n, a in slots.items()}
+    for n, a in (extra or {}).items():
+        if n.startswith(MODEL_SCOPE):
+            raise CheckpointError("%s: extra entries must lie outside %s" % (n, MODEL_SCOPE))
+        tensors[n] = np.asarray(a)
+    write_checkpoint(prefix, tensors)
+
+
+def read_slots(prefix):
+    """The two halves write_slots wrote: ({store name: momentum accumulator}, {other name: ndarray})."""
+    slots, extra = {}, {}
+    for name, arr in read_checkpoint(prefix).items():
+        if name.startswith(MODEL_SCOPE) and name.endswith(MOMENTUM_SLOT):
+            slots[name[len(MODEL_SCOPE):-len(MOMENTUM_SLOT)]] = arr
+        else:
+            extra[name] = arr
+    return slots, extra
