@@ -87,6 +87,7 @@ SYMBOLS = [
     ("d3f_momentum_clip_workspace_bytes", _Z, [_I, _LL]),
     ("d3f_momentum_clip_update", _I, [_P, _I, _LL, _F, _F, _F, _P, _Z, _P]),
     ("d3f_rank_mean", _I, [_P, _I, _LL, _P, _P]),
+    ("d3f_kernel_point_optimize", _I, [_P, _I, _I, _I, _I, _P, _P, _P, _P]),
 ]
 
 _lib = None

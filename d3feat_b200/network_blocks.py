@@ -16,7 +16,8 @@ The blocks are inference only (training = dropout_prob < 0.99 must be False, lik
 batch norm uses the moving statistics and is folded, together with the LeakyReLU and the residual add, into the
 epilogue of the producing kernel. Parameters are looked up in the active ParamStore under the reference's
 variable-scope names. The schedule of scopes, radii and widths (architecture, run_blocks) is shared with the training
-blocks (training.forward) and the seeded parameters (synth.make_params).
+blocks (training.forward); the variables it creates (variables) are shared by the seeded parameters
+(synth.make_params) and the initial parameters of a new run (training.initial_params).
 """
 from collections import namedtuple
 
@@ -302,6 +303,64 @@ def architecture(config):
         decoder.append(Step(block, layer, "uplayer_{:d}/{:s}_{:d}".format(layer, block, i), r, fdim, False, up))
         layer, r, fdim, i = (layer - 1, r * 0.5, fdim // 2, 0) if up else (layer, r, fdim, i + 1)
     return encoder, decoder
+
+
+# One variable of the schedule: its name (for kind "batch_norm" the scope of the batch norm's variables), shape and
+# kind: "weights", "kernel_points" (radius: the KPConv's 1.5 * KP_extent), "batch_norm" (shape (width,)),
+# "offset_conv_weights" or "offset_conv_bias".
+Variable = namedtuple("Variable", "name shape kind radius")
+
+
+def variables(config):
+    """The model variables of architecture(config), in creation order: what the blocks of :194-723 and
+    models/D3Feat.py:15-63 create under their scopes. synth.make_params and training.initial_params both fill this one
+    schedule."""
+    K, cin, skip_dims, out = config.num_kernel_points, config.in_features_dim, [], []
+    encoder, decoder = architecture(config)
+
+    def add(name, shape, kind, radius=None):
+        out.append(Variable(name, tuple(int(x) for x in shape), kind, radius))
+
+    for step in encoder:
+        block, scope, fdim = step.block, step.scope, step.fdim
+        if step.skip:
+            skip_dims.append(cin)
+        radius = 1.5 * config.KP_extent * step.radius / config.density_parameter
+        if block == "simple":
+            add(scope + "/weights", (K, cin, fdim), "weights")
+            add(scope + "/kernel_points", (K, 3), "kernel_points", radius)
+            add(scope, (fdim,), "batch_norm")
+            cin = fdim
+        elif block.startswith("resnetb"):
+            mid = fdim // 2
+            add(scope + "/conv1/weights", (cin, mid), "weights")
+            add(scope + "/conv1", (mid,), "batch_norm")
+            add(scope + "/conv2/weights", (K, mid, mid), "weights")
+            add(scope + "/conv2/kernel_points", (K, 3), "kernel_points", radius)
+            add(scope + "/conv2", (mid,), "batch_norm")
+            if "deformable" in block:
+                od = (4 if config.modulated else 3) * K
+                add(scope + "/conv2/offset_conv_weights", (K, mid, od), "offset_conv_weights")
+                add(scope + "/conv2/offset_conv_bias", (od,), "offset_conv_bias")
+            add(scope + "/conv3/weights", (mid, 2 * fdim), "weights")
+            add(scope + "/conv3", (2 * fdim,), "batch_norm")
+            if cin != 2 * fdim:
+                add(scope + "/shortcut/weights", (cin, 2 * fdim), "weights")
+                add(scope + "/shortcut", (2 * fdim,), "batch_norm")
+            cin = 2 * fdim
+        else:
+            raise ValueError("Unknown block name in the architecture definition : " + block)
+    for step in decoder:
+        if step.block == "unary":
+            add(step.scope + "/weights", (cin, step.fdim), "weights")
+            add(step.scope, (step.fdim,), "batch_norm")
+            cin = step.fdim
+        elif step.block == "last_unary":
+            add(step.scope + "/weights", (cin, 32), "weights")
+            cin = 32
+        if step.concat:
+            cin += skip_dims[step.layer - 1]
+    return out
 
 
 def run_blocks(steps, block_ops, inputs, features, F, config, *args):

@@ -17,7 +17,7 @@ rounded to 1e-3) under the reference's variable names.
 """
 import numpy as np
 
-from .network_blocks import architecture
+from .network_blocks import variables
 from .variables import ParamStore
 
 ARCH_3DMATCH = ["simple", "resnetb",
@@ -242,53 +242,21 @@ def _bn(rng, params, scope, dim, trained_like):
 
 
 def make_params(config, seed=0, trained_like_bn=True):
-    """Seeded weights / BN statistics / kernel points under the reference's variable scopes, walked by
-    network_blocks.architecture ('layer_{l}/{block}_{i}', 'uplayer_{l}/{block}_{i}')."""
+    """Seeded weights / BN statistics / kernel points under the reference's variable scopes, the schedule of
+    network_blocks.variables ('layer_{l}/{block}_{i}', 'uplayer_{l}/{block}_{i}')."""
     rng = np.random.default_rng(seed)
     p = {}
-    K = config.num_kernel_points
-    cin = config.in_features_dim
-    skip_dims = []
-    encoder, decoder = architecture(config)
-    for step in encoder:
-        block, scope, fdim = step.block, step.scope, step.fdim
-        if step.skip:
-            skip_dims.append(cin)
-        extent = config.KP_extent * step.radius / config.density_parameter
-        if block == "simple":
-            p[scope + "/weights"] = weight_variable(rng, (K, cin, fdim))
-            p[scope + "/kernel_points"] = kernel_points(rng, 1.5 * extent, K)
-            _bn(rng, p, scope, fdim, trained_like_bn)
-            cin = fdim
-        elif block.startswith("resnetb"):
-            mid = fdim // 2
-            p[scope + "/conv1/weights"] = weight_variable(rng, (cin, mid))
-            _bn(rng, p, scope + "/conv1", mid, trained_like_bn)
-            p[scope + "/conv2/weights"] = weight_variable(rng, (K, mid, mid))
-            p[scope + "/conv2/kernel_points"] = kernel_points(rng, 1.5 * extent, K)
-            _bn(rng, p, scope + "/conv2", mid, trained_like_bn)
-            if "deformable" in block:
-                od = (4 if config.modulated else 3) * K
-                # the reference initialises the offset head to zero (convolution_ops.py:327-328); small
-                # non-zero seeds are used so that the deformed path is actually exercised
-                p[scope + "/conv2/offset_conv_weights"] = (0.02 * weight_variable(rng, (K, mid, od))).astype(np.float32)
-                p[scope + "/conv2/offset_conv_bias"] = rng.normal(scale=0.01, size=od).astype(np.float32)
-            p[scope + "/conv3/weights"] = weight_variable(rng, (mid, 2 * fdim))
-            _bn(rng, p, scope + "/conv3", 2 * fdim, trained_like_bn)
-            if cin != 2 * fdim:
-                p[scope + "/shortcut/weights"] = weight_variable(rng, (cin, 2 * fdim))
-                _bn(rng, p, scope + "/shortcut", 2 * fdim, trained_like_bn)
-            cin = 2 * fdim
-        else:
-            raise ValueError("Unknown block name in the architecture definition : " + block)
-    for step in decoder:
-        if step.block == "unary":
-            p[step.scope + "/weights"] = weight_variable(rng, (cin, step.fdim))
-            _bn(rng, p, step.scope, step.fdim, trained_like_bn)
-            cin = step.fdim
-        elif step.block == "last_unary":
-            p[step.scope + "/weights"] = weight_variable(rng, (cin, 32))
-            cin = 32
-        if step.concat:
-            cin += skip_dims[step.layer - 1]
+    for v in variables(config):
+        if v.kind == "weights":
+            p[v.name] = weight_variable(rng, v.shape)
+        elif v.kind == "kernel_points":
+            p[v.name] = kernel_points(rng, v.radius, v.shape[0])
+        elif v.kind == "batch_norm":
+            _bn(rng, p, v.name, v.shape[0], trained_like_bn)
+        elif v.kind == "offset_conv_weights":
+            # the reference initialises the offset head to zero (convolution_ops.py:327-328); small non-zero seeds
+            # are used so that the deformed path is actually exercised
+            p[v.name] = (0.02 * weight_variable(rng, v.shape)).astype(np.float32)
+        elif v.kind == "offset_conv_bias":
+            p[v.name] = rng.normal(scale=0.01, size=v.shape).astype(np.float32)
     return p

@@ -1,7 +1,7 @@
 """Training graph of D3Feat on the GPU: the rigid blocks of models/network_blocks.py and the decoder of
 models/D3Feat.py with training = True, and the loss of models/KPFCNN_model.py:142-188 / utils/loss.py.
 
-    store = ParamStore(params, "cuda")
+    store = ParamStore(training.initial_params(config, seed), "cuda")   # or a restored snapshot
     params = training.trainable(store)               # weights, gamma, beta, offset require grad
     opt = training.MomentumClip(params, config.learning_rate, config.momentum, config.grad_clip_norm)
     with use_params(store):
@@ -398,6 +398,51 @@ def forward(inputs, config):
     features = nb.run_blocks(encoder, get_block_ops, inputs, inputs["features"], F, config)
     features = nb.run_blocks(decoder, get_block_ops, inputs, features, F, config)
     return l2_normalize(features), detection_scores(features, inputs["neighbors"][0], inputs["lengths"][0])
+
+
+def initial_params(config, seed=0):
+    """The variables a new run of the reference starts from, {name: float32 array} under the schedule of
+    network_blocks.variables (ready for ParamStore):
+      weights              weight_variable (models/network_blocks.py:37-41): normal with std sqrt(2 / shape[-1]),
+                           redrawn beyond 2 std (tf.truncated_normal), then round(x * 1000) / 1000, in float32
+      batch norm           gamma 1, beta 0, moving mean 0, moving variance 1 (tf.layers.batch_normalization); with
+                           config.use_batch_norm off the '<scope>/offset' bias, 0 (:162-165)
+      offset_conv_*        0 (kernels/convolution_ops.py:327-328)
+      kernel_points        kernel_points.load_kernels(1.5 * KP_extent, K, 1, 3, config.fixed_kernel_points): one
+                           disposition optimised once for the run, each KPConv with its own rotation and noise
+                           (kernels/convolution_ops.py:127-148)
+    Draws are counter-based splitmix64 of `seed` (kernel_points.draw), so a seed gives the same bits everywhere; numpy's
+    and TF's random streams are not reproduced."""
+    from . import kernel_points as kp
+    K, fixed = config.num_kernel_points, config.fixed_kernel_points
+    D = None
+    p = {}
+    for i, v in enumerate(nb.variables(config)):
+        if v.kind == "weights":
+            n = int(np.prod(v.shape))
+            e = np.arange(n, dtype=np.uint64) * np.uint64(64)
+            z = kp.normal(kp.sub_seed(seed, i), kp.WEIGHTS, e).astype(np.float32)
+            for a in range(1, 64):                        # tf.truncated_normal redraws beyond 2 std
+                bad = np.nonzero(np.abs(z) > 2)[0]
+                if bad.size == 0:
+                    break
+                z[bad] = kp.normal(kp.sub_seed(seed, i), kp.WEIGHTS, e[bad] + np.uint64(a)).astype(np.float32)
+            w = z * np.float32(np.sqrt(2 / v.shape[-1]))
+            p[v.name] = (np.round(w * np.float32(1000)) / np.float32(1000)).astype(np.float32).reshape(v.shape)
+        elif v.kind == "kernel_points":
+            if D is None:
+                D = kp.shared_disposition(K, fixed, seed)
+            p[v.name] = kp.load_kernels(v.radius, K, 1, 3, fixed, seed=kp.sub_seed(seed, i), disposition=D)[0].astype(
+                np.float32)
+        elif v.kind == "batch_norm":
+            if config.use_batch_norm:
+                for name, x in zip(V.ParamStore.bn_names(v.name), (1, 0, 0, 1)):
+                    p[name] = np.full(v.shape, x, np.float32)
+            else:
+                p[v.name + "/offset"] = np.zeros(v.shape, np.float32)
+        else:                                             # offset_conv_weights, offset_conv_bias
+            p[v.name] = np.zeros(v.shape, np.float32)
+    return p
 
 
 def trainable(store):

@@ -48,6 +48,8 @@
  *   d3f_momentum_clip_update  utils/trainer.py:116-156 (tf.clip_by_norm per gradient + tf.train.MomentumOptimizer)
  *   d3f_rank_mean             the data-parallel mean of gradients and batch statistics over ranks (no counterpart:
  *                             the reference trains on one GPU)
+ *   d3f_kernel_point_optimize kernels/kernel_points.py:102-174 (kernel_point_optimization_debug: the potential-minimising
+ *                             kernel-point dispositions load_kernels starts a run from)
  */
 #ifndef D3FEAT_B200_H_
 #define D3FEAT_B200_H_
@@ -654,6 +656,32 @@ int d3f_momentum_clip_update(const d3f_momentum_tensor* table, int T, long long 
                              float momentum, float clip_norm, void* workspace, size_t workspace_bytes,
                              d3f_stream_t stream);
 int d3f_rank_mean(const float* x, int R, long long P, float* out, d3f_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * The kernel-point optimiser (kernels/kernel_points.py:102-174). Contract: oracle/kernel_points_np.py (optimize),
+ * exactly. initial[T, K, 3] (device, fp64) are T tries of K points, already fixed as :85-91 fixes them (fixed =
+ * D3F_FIXED_*: point 0 at the origin for CENTER; points 0-2 at 0 and +-2/3 on z for VERTICALS). Per iteration, in fp64,
+ * one correctly rounded operation at a time, no fused multiply-add:
+ *   d2    = (dx*dx + dy*dy) + dz*dz for d = p_i - p_j;  den = d2 * sqrt(d2) + 1e-6  (the reference's d2^(3/2) via pow is
+ *           the one deviation: pow is not correctly rounded)
+ *   g_j   = (sum over i = 0..K-1, in that order, of (p_i - p_j) / den) + 10 * p_j;  VERTICALS: g_1, g_2 lose x and y
+ *   n_j   = sqrt(((gx*gx + gy*gy) + gz*gz) + 1e-12);  saved_gradient_norms[it, t] = max over the try's points of n_j
+ *   stop  when the max over all tries and the moving points (j >= 1 CENTER, j >= 3 VERTICALS, all NONE) of
+ *         |n_j(previous iteration) - n_j| < 1e-5 (the previous norms start at 0)
+ *   move  m_j = min(mf * n_j, 0.05), 0 for j = 0 unless NONE;  p_j -= (m_j * g_j) / (n_j + 1e-6);  mf *= 0.9995 (from 1e-2)
+ * at most 10000 iterations. Outputs (device): points[T, K, 3] the final points, before the reference's rescale (:177-181);
+ * saved_gradient_norms[10000, T], zero from row *iterations on; *iterations (int) the rows written. No point moves when
+ * K <= 1 (CENTER) or K <= 3 (VERTICALS): then no iteration runs (the reference fails on an empty maximum), the points
+ * are copied and *iterations = 0. points must not overlap initial. One CTA runs the whole loop (T*K <= 6400, 200 KB of
+ * shared memory), after one memset of saved_gradient_norms; no host synchronisation, no atomics: bitwise identical run
+ * to run and across streams. dimension != 3, an unknown fixed, T < 1, K < 1, T*K > 6400 or a null pointer:
+ * D3F_ERR_INVALID before any CUDA call.
+ * ------------------------------------------------------------------------------------------- */
+#define D3F_FIXED_NONE 0
+#define D3F_FIXED_CENTER 1
+#define D3F_FIXED_VERTICALS 2
+int d3f_kernel_point_optimize(const double* initial, int T, int K, int dimension, int fixed, double* points,
+                              double* saved_gradient_norms, int* iterations, d3f_stream_t stream);
 
 #ifdef __cplusplus
 }
