@@ -66,6 +66,8 @@ SYMBOLS = [
     ("d3f_detection_scores_backward", _I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P]),
     ("d3f_select_keypoints_workspace_bytes", _Z, [_I, _I]),
     ("d3f_select_keypoints", _I, [_P, _P, _I, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _Z, _P, _P]),
+    ("d3f_sample_keypoints_workspace_bytes", _Z, [_I]),
+    ("d3f_sample_keypoints", _I, [_P, _I, _I, _I, _U64, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _Z, _P, _P]),
     ("d3f_match_descriptors_workspace_bytes", _Z, [_I, _I]),
     ("d3f_match_descriptors", _I, [_P, _P, _I, _I, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _Z, _P]),
     ("d3f_register_pairs_workspace_bytes", _Z, [_I, _I, _I, _I]),

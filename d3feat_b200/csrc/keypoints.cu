@@ -7,7 +7,14 @@
 // min(k, len_b) of them. Canonicalising the scores first (every NaN -> one positive quiet NaN, -0.0 -> +0.0) makes
 // the order that of np.argsort(kind="stable"): NaNs above +inf, ties by ascending row. All launches are sized by the
 // capacity and read the row count from n_dev, so the whole selection can be captured in a CUDA graph.
+//
+// Random keypoints for the same layout -- the testers' `-rand` arm: np.random.choice(len, k) per cloud, with
+// replacement (utils/tester.py:238-279, geometric_registration/evaluate.py:45-54) -- are counter-based draws of
+// rng.cuh, one per output slot (d3f_sample_keypoints).
+#include <climits>
+
 #include "ops.cuh"
+#include "rng.cuh"
 #include "sort.cuh"
 
 namespace d3f {
@@ -60,6 +67,37 @@ keypoint_gather_kernel(const uint32_t* __restrict__ sorted, int Ncap, const int*
     if (out_points && lane < 3) out_points[w * 3 + lane] = real ? points[(size_t)idx * 3 + lane] : 0.f;
     if (out_desc)
       for (int c = lane; c < D; c += 32) out_desc[w * D + c] = real ? desc[(size_t)idx * D + c] : 0.f;
+  }
+}
+
+// Uniform random keypoints, with replacement: slot j of cloud b holds row s_b + draw_index(z, n_b) with
+// z = splitmix64(seed + ((b << 32) | j) * golden), so a slot's row depends only on (seed, b, j, n_b) and the first c
+// slots of a k-slot draw are the c-slot draw. One warp per output slot, as keypoint_gather_kernel; the clouds are cut
+// at n as there, and an empty cloud gets count 0, index -1 and zero rows.
+__global__ void __launch_bounds__(256)
+keypoint_sample_kernel(int Ncap, const int* __restrict__ n_dev, const int* __restrict__ start, int B, int k,
+                       unsigned long long seed, const float* __restrict__ scores, const float* __restrict__ points,
+                       const float* __restrict__ desc, int D, int* __restrict__ out_index, int* __restrict__ out_count,
+                       float* __restrict__ out_points, float* __restrict__ out_desc, float* __restrict__ out_scores) {
+  const int N = dyn_rows(Ncap, n_dev);
+  const int lane = threadIdx.x & 31;
+  const long long slots = (long long)B * k;
+  const long long stride = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long w = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < slots; w += stride) {
+    const int b = (int)(w / k), j = (int)(w - (long long)b * k);
+    const int s = min(max(start[b], 0), N);
+    const int e = min(max(start[b + 1], s), N);
+    const bool real = e > s;
+    const unsigned long long c = ((unsigned long long)(unsigned)b << 32) | (unsigned)j;
+    const int idx = real ? s + draw_index(splitmix64(seed + c * kGolden), e - s) : -1;
+    if (lane == 0) {
+      if (out_index) out_index[w] = idx;
+      if (out_scores) out_scores[w] = real ? scores[idx] : 0.f;
+      if (out_count && j == 0) out_count[b] = real ? k : 0;
+    }
+    if (out_points && lane < 3) out_points[w * 3 + lane] = real ? points[(size_t)idx * 3 + lane] : 0.f;
+    if (out_desc)
+      for (int ch = lane; ch < D; ch += 32) out_desc[w * D + ch] = real ? desc[(size_t)idx * D + ch] : 0.f;
   }
 }
 
@@ -128,5 +166,44 @@ extern "C" int d3f_select_keypoints(const float* scores, const int* lengths, int
                                                        D, out_index, out_count, out_points, out_descriptors, out_scores);
     D3F_LAUNCH_CHECK("keypoint_gather_kernel");
   }
+  return D3F_OK;
+}
+
+extern "C" size_t d3f_sample_keypoints_workspace_bytes(int B) {
+  if (B < 1) return 0;
+  return align_up(sizeof(int) * ((size_t)B + 1), 256);
+}
+
+extern "C" int d3f_sample_keypoints(const int* lengths, int B, int N, int k, uint64_t seed, const float* points,
+                                    const float* descriptors, int D, const float* scores, int* out_index,
+                                    int* out_count, float* out_points, float* out_descriptors, float* out_scores,
+                                    void* workspace, size_t workspace_bytes, d3f_stream_t stream_, const int* n_dev) {
+  cudaStream_t stream = (cudaStream_t)stream_;
+  D3F_REQUIRE(B >= 1 && B <= kMaxBatch, D3F_ERR_INVALID, "sample_keypoints: B=%d must be in [1,%d]", B, kMaxBatch);
+  D3F_REQUIRE(N >= 0, D3F_ERR_INVALID, "sample_keypoints: bad shape N=%d", N);
+  D3F_REQUIRE(k >= 1 && (long long)B * k <= INT_MAX, D3F_ERR_INVALID,
+              "sample_keypoints: k=%d must be >= 1 with B*k=%lld within int32", k, (long long)B * k);
+  D3F_REQUIRE(out_index || out_count || out_points || out_descriptors || out_scores, D3F_ERR_INVALID,
+              "sample_keypoints: no output requested");
+  D3F_REQUIRE(descriptors == nullptr || D >= 1, D3F_ERR_INVALID, "sample_keypoints: D=%d must be >= 1", D);
+  D3F_REQUIRE(out_points == nullptr || points != nullptr, D3F_ERR_INVALID,
+              "sample_keypoints: gathered points requested without points");
+  D3F_REQUIRE(out_descriptors == nullptr || descriptors != nullptr, D3F_ERR_INVALID,
+              "sample_keypoints: gathered descriptors requested without descriptors");
+  D3F_REQUIRE(out_scores == nullptr || scores != nullptr, D3F_ERR_INVALID,
+              "sample_keypoints: gathered scores requested without scores");
+  D3F_REQUIRE(lengths != nullptr && workspace != nullptr, D3F_ERR_INVALID, "sample_keypoints: null pointer");
+  D3F_REQUIRE(workspace_bytes >= d3f_sample_keypoints_workspace_bytes(B), D3F_ERR_WORKSPACE,
+              "sample_keypoints: workspace too small");
+  Carver cv(workspace, workspace_bytes);
+  int* start = cv.take<int>((size_t)B + 1);
+  int rc = launch_batch_start(lengths, B, start, stream);
+  if (rc) return rc;
+  const long long slots = (long long)B * k;
+  const int blocks = (int)min((slots + 7) / 8, (long long)16 * kNumSMs);
+  keypoint_sample_kernel<<<blocks, 256, 0, stream>>>(N, n_dev, start, B, k, (unsigned long long)seed, scores, points,
+                                                     descriptors, D, out_index, out_count, out_points, out_descriptors,
+                                                     out_scores);
+  D3F_LAUNCH_CHECK("keypoint_sample_kernel");
   return D3F_OK;
 }

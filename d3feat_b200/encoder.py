@@ -15,7 +15,7 @@ import torch
 from . import network_blocks as nb
 from . import pyramid
 from .evaluation import OPTIONS as EVALUATE_OPTIONS, GroundTruth, check_evaluate_options, check_truth, evaluate_pairs
-from .keypoints import select_keypoints
+from .keypoints import sample_keypoints, select_keypoints
 from .matching import host_pairs, match_keypoints
 from .registration import ICP_OPTIONS, OPTIONS as REGISTER_OPTIONS, check_icp_options, check_options, icp_pairs, \
     register_pairs
@@ -34,6 +34,45 @@ RefinedDetections = namedtuple("RefinedDetections", "descriptors scores keypoint
 # registration / refinement are None when the pipeline does not run them
 EvaluatedDetections = namedtuple("EvaluatedDetections",
                                  "descriptors scores keypoints matches registration refinement evaluation")
+# GraphPipeline(..., match_pairs=pairs, sweep={...}) result: the fields above (None for the stages the pipeline does not
+# run) plus sweep, a dict (arm, count) -> SweepEntry in the order of sweep_arms x sweep_counts
+SweptDetections = namedtuple("SweptDetections",
+                             "descriptors scores keypoints matches registration refinement evaluation sweep")
+SweepEntry = namedtuple("SweepEntry", "keypoints matches registration refinement evaluation")
+SWEEP_ARMS = ("score", "random")
+SWEEP_OPTIONS = ("counts", "arms", "seed")
+
+
+def check_sweep(sweep, keypoints, who="GraphPipeline"):
+    """(counts, arms, seed) of a sweep={...} option, or ValueError: counts strictly descending within [1, keypoints],
+    arms a non-empty subset of SWEEP_ARMS without repeats (default both), seed an integer in [0, 2^64) (default 0)."""
+    if not isinstance(sweep, dict) or set(sweep) - set(SWEEP_OPTIONS) or "counts" not in sweep:
+        raise ValueError("%s: sweep must be a dict of %s with counts, got %r" % (who, SWEEP_OPTIONS, sweep))
+
+    def is_int(x):
+        return not isinstance(x, bool) and isinstance(x, (int, np.integer))
+    try:
+        counts = tuple(sweep["counts"])
+    except TypeError:
+        counts = None
+    if not counts or not all(is_int(c) for c in counts):
+        raise ValueError("%s: sweep counts=%r must be a non-empty sequence of integers" % (who, sweep["counts"]))
+    counts = tuple(int(c) for c in counts)
+    if any(b >= a for a, b in zip(counts, counts[1:])) or not 1 <= counts[-1] or counts[0] > keypoints:
+        raise ValueError("%s: sweep counts=%r must descend strictly within [1, keypoints=%d]" % (who, counts,
+                                                                                                 keypoints))
+    arms = sweep.get("arms", SWEEP_ARMS)
+    arms = (arms,) if isinstance(arms, str) else arms
+    try:
+        arms = tuple(arms)
+    except TypeError:
+        arms = ()
+    if not arms or any(a not in SWEEP_ARMS for a in arms) or len(set(arms)) != len(arms):
+        raise ValueError("%s: sweep arms=%r must be a non-empty subset of %s" % (who, sweep.get("arms"), SWEEP_ARMS))
+    seed = sweep.get("seed", 0)
+    if not is_int(seed) or not 0 <= int(seed) < 2 ** 64:
+        raise ValueError("%s: sweep seed=%r must be an integer in [0, 2^64)" % (who, seed))
+    return counts, arms, int(seed)
 
 
 class KPFCNN:
@@ -254,18 +293,37 @@ class GraphPipeline:
     level 0 (points, lengths, row count) on the device: raw scans in, the reference's voxel_down_sample(v) input stage
     inside the graph, no host step. Capacities and bbox are those of the voxelised level 0 (for_batch sizes them from
     one voxelised batch); more voxels than capacities[0] set status bit 1, a cloud wider than the bbox allows bit 0.
-    Keypoints, ICP and the evaluation see the voxelised level 0."""
+    Keypoints, ICP and the evaluation see the voxelised level 0.
+
+    sweep=dict(counts=(5000, 2500, 1000, 500, 250), arms=("score", "random"), seed=0) (needs match_pairs): D3Feat's
+    keypoint-count experiment, the testers' `-pred` and `-rand` arms. counts descend strictly and are at most
+    keypoints; arms is a non-empty subset of ("score", "random"). The encoder graph then also runs, for every (arm,
+    count), the pipeline's matching, registration, ICP and evaluation on that arm's keypoint set, and `res` is a
+    SweptDetections: the fields of the pipeline's regular result plus sweep, a dict (arm, count) -> SweepEntry(keypoints,
+    matches, registration, refinement, evaluation). The score arm at count c is select_keypoints(k=c), exactly the
+    keypoints of a pipeline built with keypoints=c. The random arm draws counts[0] uniform slots per cloud, with
+    replacement (keypoints.sample_keypoints with the sweep's seed, one draw per step and cloud, shared by every pair of
+    the cloud); count c is its first c slots, which sample_keypoints(k=c) gathers directly (each slot is its own draw).
+    With evaluate, the repeatability levels are checked against the smallest count, and every stage, the regular result
+    included, uses them; evaluation_totals() is then [len(arms), len(counts), n_tot], for evaluation.sweep_summary(totals,
+    pipe.sweep_arms, pipe.sweep_counts, pipe.evaluate_levels, pipe.evaluate_pose_sets)."""
 
     DEPTH = 4
 
     def __init__(self, enc, capacities, n_clouds, bbox, decoder=False, post=None, encoder_streams=2, keypoints=None,
-                 match_pairs=None, register=None, icp=None, evaluate=None, voxel_size=None, raw_capacity=None):
+                 match_pairs=None, register=None, icp=None, evaluate=None, voxel_size=None, raw_capacity=None,
+                 sweep=None):
         if keypoints is not None and not decoder:
             raise ValueError("GraphPipeline: keypoints=%r needs decoder=True (the detection scores)" % (keypoints,))
         if keypoints is not None and int(keypoints) < 1:
             raise ValueError("GraphPipeline: keypoints=%r must be >= 1" % (keypoints,))
         if match_pairs is not None and keypoints is None:
             raise ValueError("GraphPipeline: match_pairs needs keypoints=k (the descriptors it matches)")
+        self.sweep_counts = self.sweep_arms = self.sweep_seed = None
+        if sweep is not None:
+            if match_pairs is None:
+                raise ValueError("GraphPipeline: sweep needs match_pairs (the pairs every keypoint count is matched on)")
+            self.sweep_counts, self.sweep_arms, self.sweep_seed = check_sweep(sweep, int(keypoints))
         if voxel_size is not None and raw_capacity is None:
             raise ValueError("GraphPipeline: voxel_size needs raw_capacity (the raw rows a slot holds)")
         if register is not None:
@@ -288,9 +346,12 @@ class GraphPipeline:
             if not isinstance(evaluate, dict) or set(evaluate) - set(EVALUATE_OPTIONS):
                 raise ValueError("GraphPipeline: evaluate must be a dict of evaluate_pairs options %s, got %r" % (
                     EVALUATE_OPTIONS, evaluate))
-            self.evaluate_levels = check_evaluate_options(int(keypoints), **evaluate, who="GraphPipeline")[0]
+            k_min = int(keypoints) if sweep is None else self.sweep_counts[-1]
+            self.evaluate_levels = check_evaluate_options(k_min, **evaluate, who="GraphPipeline")[0]
             self.evaluate_pose_sets = ("ransac",) * (register is not None) + ("icp",) * (icp is not None)
         self.evaluate = None if evaluate is None else dict(evaluate)
+        if sweep is not None and evaluate is not None:
+            self.evaluate["repeat_levels"] = self.evaluate_levels     # one set of levels for every count
         self.icp = None if icp is None else dict(icp)
         pairs = None if match_pairs is None else host_pairs(match_pairs, int(n_clouds), "GraphPipeline")
         self.register = None if register is None else dict(register)
@@ -330,7 +391,9 @@ class GraphPipeline:
                                       torch.zeros((P, 6, 6), dtype=f64, device=dev),
                                       torch.zeros((P,), dtype=torch.int32, device=dev)) for _ in range(self.DEPTH)]
             n_tot = 4 + len(self.evaluate_levels) + 7 * len(self.evaluate_pose_sets)
-            self.eval_running = torch.zeros((n_tot,), dtype=f64, device=dev)
+            shape = (n_tot,) if sweep is None else (len(self.sweep_arms), len(self.sweep_counts), n_tot)
+            self.eval_running = torch.zeros(shape, dtype=f64, device=dev)
+            self.sweep_totals = [None] * self.DEPTH     # per slot: the step's sweep totals, stacked in the graph
 
     @classmethod
     def for_batch(cls, enc, points, lengths, slack=1.125, margin=0.05, **kw):
@@ -368,27 +431,55 @@ class GraphPipeline:
             kp = select_keypoints(scores, inputs["lengths"][0], self.keypoints, points=inputs["points"][0],
                                   descriptors=desc, rows=inputs["rows"][0])
             if self.match_pairs is not None:
-                m = match_keypoints(kp, self.match_pairs)
-                if self.evaluate is not None:
-                    reg = ref = None
-                    if self.register is not None:
-                        reg = register_pairs(kp, m, self.match_pairs, **self.register)
-                        if self.icp is not None:
-                            ref = icp_pairs(inputs["points"][0], inputs["lengths"][0], self.match_pairs, reg.pose,
-                                            rows=inputs["rows"][0], bbox=self.bbox, **self.icp)
-                    ev = evaluate_pairs(kp, m, self.match_pairs, self.truth[k], reg, ref, **self.evaluate)
+                m, reg, ref, ev = self._run_pairs(inputs, k, kp)
+                if self.sweep_counts is not None:
+                    return F, self._run_sweep(inputs, k, desc, scores, SweepEntry(kp, m, reg, ref, ev))
+                if ev is not None:
                     return F, EvaluatedDetections(desc, scores, kp, m, reg, ref, ev)
-                if self.register is not None:
-                    reg = register_pairs(kp, m, self.match_pairs, **self.register)
-                    if self.icp is not None:
-                        ref = icp_pairs(inputs["points"][0], inputs["lengths"][0], self.match_pairs, reg.pose,
-                                        rows=inputs["rows"][0], bbox=self.bbox, **self.icp)
-                        return F, RefinedDetections(desc, scores, kp, m, reg, ref)
+                if ref is not None:
+                    return F, RefinedDetections(desc, scores, kp, m, reg, ref)
+                if reg is not None:
                     return F, RegisteredDetections(desc, scores, kp, m, reg)
                 return F, MatchedDetections(desc, scores, kp, m)
             return F, Detections(desc, scores, kp)
         res = self.enc.describe(inputs, F) if self.decoder else F[-1]
         return F, res
+
+    def _run_pairs(self, inputs, k, kp):
+        """(matches, registration, refinement, evaluation) of the match pairs on the keypoint set kp, None for the
+        stages the pipeline does not run."""
+        m = match_keypoints(kp, self.match_pairs)
+        reg = ref = ev = None
+        if self.register is not None:
+            reg = register_pairs(kp, m, self.match_pairs, **self.register)
+            if self.icp is not None:
+                ref = icp_pairs(inputs["points"][0], inputs["lengths"][0], self.match_pairs, reg.pose,
+                                rows=inputs["rows"][0], bbox=self.bbox, **self.icp)
+        if self.evaluate is not None:
+            ev = evaluate_pairs(kp, m, self.match_pairs, self.truth[k], reg, ref, **self.evaluate)
+        return m, reg, ref, ev
+
+    def _run_sweep(self, inputs, k, desc, scores, main):
+        """Every (arm, count) of the sweep on slot k, after the regular result `main` (a SweepEntry). The score arm at
+        count == keypoints is `main` itself; the random arm's count c is the first c slots of the counts[0] draw, drawn
+        directly with k=c."""
+        pts, lens, rows = inputs["points"][0], inputs["lengths"][0], inputs["rows"][0]
+        entries = {}
+        for arm in self.sweep_arms:
+            for c in self.sweep_counts:
+                if arm == "score" and c == self.keypoints:
+                    entries[(arm, c)] = main
+                    continue
+                if arm == "score":
+                    kp = select_keypoints(scores, lens, c, points=pts, descriptors=desc, rows=rows)
+                else:
+                    kp = sample_keypoints(lens, c, self.sweep_seed, points=pts, descriptors=desc, scores=scores,
+                                          rows=rows)
+                entries[(arm, c)] = SweepEntry(kp, *self._run_pairs(inputs, k, kp))
+        if self.evaluate is not None:
+            self.sweep_totals[k] = torch.stack([e.evaluation.totals for e in entries.values()]).view(
+                self.eval_running.shape)
+        return SweptDetections(desc, scores, *main, entries)
 
     def _capture(self, k):
         """Eager warm-up of both halves on slot k (lazy one-time work: weight packing, BN folding, kernel attributes,
@@ -515,7 +606,8 @@ class GraphPipeline:
         if self.evaluate is not None:
             # on the caller's stream, after this step's encoder: consecutive encoders may overlap on their two
             # streams, so the running totals are never written inside a graph
-            self.eval_running.add_(self.out[k][2].evaluation.totals)
+            self.eval_running.add_(self.out[k][2].evaluation.totals if self.sweep_counts is None else
+                                   self.sweep_totals[k])
         self.pending = (self._load(next_points, next_lengths, inputs_ready, next_truth)
                         if next_points is not None else None)
         return res, self.slots[k].counts
@@ -524,13 +616,14 @@ class GraphPipeline:
         """The running totals of every step since construction or reset_evaluation(), as float64 numpy (one
         device->host read on the caller's stream, after the pyramid of the pending batch): see evaluation.summary.
         Raises RuntimeError, as check() does, once any batch loaded so far has overflowed the bucket: its totals
-        were computed on truncated clouds."""
+        were computed on truncated clouds. With sweep the totals are [len(sweep_arms), len(sweep_counts), n_tot]."""
         cur = torch.cuda.current_stream(self.enc.device)
         cur.wait_stream(self.s_pyr)
         status = torch.cat([buf.status for buf in self.slots]).to(torch.float64)
-        got = torch.cat([self.eval_running, status]).cpu().numpy()
-        self._raise_on_status(got[self.eval_running.shape[0]:].astype(np.int64))
-        return got[:self.eval_running.shape[0]]
+        n = self.eval_running.numel()
+        got = torch.cat([self.eval_running.reshape(-1), status]).cpu().numpy()
+        self._raise_on_status(got[n:].astype(np.int64))
+        return got[:n].reshape(self.eval_running.shape)
 
     def reset_evaluation(self):
         """Zero the running totals. The status words stay set: see check()."""

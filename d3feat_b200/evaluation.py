@@ -208,3 +208,16 @@ def summary(totals, levels, pose_sets=("ransac",)):
         out[name] = dict(successes=int(b[0]), success_rate=div(b[0], n), rte=div(b[1], b[2]), rre_deg=div(b[3], b[4]),
                          recall_hits=int(b[5]), recall_pairs=int(b[6]), registration_recall=div(b[5], b[6]))
     return out
+
+
+def sweep_summary(totals, arms, counts, levels, pose_sets=("ransac",)):
+    """The keypoint-count table of a GraphPipeline(..., sweep=...) run: one row per (arm, count), arms outer, each the
+    summary() of that row's totals plus its "arm" and "count" -- inlier ratio, FMR, repeatability, and per pose set the
+    success rate, RTE, RRE and registration recall. totals [len(arms), len(counts), 4 + R + 7 S] (evaluation_totals())."""
+    t = np.asarray(totals.cpu() if torch.is_tensor(totals) else totals, np.float64)
+    arms, counts = tuple(arms), tuple(int(c) for c in counts)
+    if t.ndim != 3 or t.shape[:2] != (len(arms), len(counts)):
+        raise ValueError("sweep_summary: totals of shape %s for %d arms and %d counts" % (t.shape, len(arms),
+                                                                                         len(counts)))
+    return [dict(arm=a, count=c, **summary(t[i, j], levels, pose_sets))
+            for i, a in enumerate(arms) for j, c in enumerate(counts)]

@@ -31,6 +31,8 @@
  *   d3f_closest_pool          models/network_blocks.py:69-83
  *   d3f_l2_normalize          models/D3Feat.py:65
  *   d3f_select_keypoints      utils/tester.py:209-213, 281-290 (host argsort of the detection scores)
+ *   d3f_sample_keypoints      utils/tester.py:238-279, geometric_registration/evaluate.py:45-54 (np.random.choice of
+ *                             the `-rand` keypoints)
  *   d3f_match_descriptors     geometric_registration/evaluate.py:11-27 (build_correspondence: mutual nearest
  *                             neighbours of two fragments' keypoint descriptors)
  *   d3f_register_pairs        geometric_registration/evaluate.py:84-99, utils/tester.py:305-316,
@@ -428,6 +430,22 @@ int d3f_detection_scores_backward(const float* feats, const int* neighbors, cons
 size_t d3f_select_keypoints_workspace_bytes(int N, int B);
 int d3f_select_keypoints(const float* scores, const int* lengths, int B, int N, int k, const float* points,
                          const float* descriptors, int D, int* out_order, int* out_index, int* out_count,
+                         float* out_points, float* out_descriptors, float* out_scores, void* workspace,
+                         size_t workspace_bytes, d3f_stream_t stream, const int* n_dev);
+
+/* Uniform random keypoints of B stacked clouds, with replacement (the testers' `-rand` arm: np.random.choice(len_b, k)
+ * per cloud, utils/tester.py:238-279, geometric_registration/evaluate.py:45-54), in the d3f_select_keypoints layout.
+ *   lengths[B] (device), optional points[N,3], descriptors[N,D], scores[N] (N = capacity with n_dev).
+ *   Cloud b holds rows [s_b, e_b) = [start_b, start_b + len_b) cut at n; n_b = e_b - s_b. For every slot j < k:
+ *     c = (b << 32) | j, z = splitmix64(seed + c * 0x9E3779B97F4A7C15), out_index[b,j] = s_b + (((z >> 32) * n_b) >> 32)
+ *   (uint64, wrapping): draws are independent per slot, so the first c slots of a k-slot draw are the c-slot draw.
+ *   out_count[b] = k when n_b >= 1; an empty cloud gets count 0, index -1 and zero rows. Rows of no cloud are never
+ *   drawn; a row may be drawn more than once. out_points[B,k,3], out_descriptors[B,k,D], out_scores[B,k] gather the
+ *   drawn rows (each optional, at least one output required). 1 <= B <= 1024, k >= 1 with B*k <= INT32_MAX, D >= 1
+ *   with descriptors. Graph-capturable. */
+size_t d3f_sample_keypoints_workspace_bytes(int B);
+int d3f_sample_keypoints(const int* lengths, int B, int N, int k, uint64_t seed, const float* points,
+                         const float* descriptors, int D, const float* scores, int* out_index, int* out_count,
                          float* out_points, float* out_descriptors, float* out_scores, void* workspace,
                          size_t workspace_bytes, d3f_stream_t stream, const int* n_dev);
 
