@@ -383,7 +383,10 @@ sample_pick_kernel(const long long* __restrict__ offset, const int* __restrict__
   if (m == 0) valid[p] = ok;
   int a = -1, b = -1;
   if (ok) {
-    const unsigned c = replace ? (unsigned)draw_index(draw(seed, p, (unsigned)m, kSlotDraw), n) : sorted[lo + m];
+    // rows before offset[0] belong to no pair and sort last, so pair p's candidates sit at lo - offset[0] in `sorted`
+    const long long lo0 = min(max(offset[0], 0ll), (long long)M);
+    const unsigned c = replace ? (unsigned)draw_index(draw(seed, p, (unsigned)m, kSlotDraw), n)
+                               : sorted[(lo - lo0) + m];
     if (c < (unsigned)n) {
       a = rows[2 * (lo + c)];
       b = rows[2 * (lo + c) + 1] + __ldg(anchor_len + p);

@@ -139,8 +139,10 @@ def correspondences(points, lengths, pairs, trans, distance, mode, *, bbox=None)
 
 
 def sample_correspondences(corr, k, replace, min_count, seed, anchor_lengths):
-    """k correspondences of every pair from corr (a Correspondences, or any table with offset [P+1] int64 from 0 to M,
-    nondecreasing, and rows [M,2] int32, such as 3DMatch's keypts.pkl converted). replace=True: k draws with
+    """k correspondences of every pair from corr (a Correspondences, or any table with offset [P+1] int64,
+    nondecreasing within [0, M], and rows [M,2] int32, such as 3DMatch's keypts.pkl converted). offset may start above
+    0 and end below M, as offset[a:b+1] of a larger table over its full rows does: rows outside [offset[0], offset[P])
+    belong to no pair. replace=True: k draws with
     replacement (ThreeDMatch.py:218-229); False: a uniform random k-subset in random order (KITTI.py:184-189).
     valid = at least max(min_count, 1) candidates and, without replacement, at least k. anchor_lengths [P] int32 (the
     anchor's rows) offsets pos into the pair's [anchor || positive] stack. Never synchronises. Returns Sample."""

@@ -600,7 +600,8 @@ int d3f_evaluate_pairs(const float* points, const int* count, int B, int k, cons
  *   cells of the origin; otherwise, or for a null pointer, D3F_ERR_INVALID before any CUDA call (the workspace query
  *   returns 0).
  * Sampling, d3f_sample_correspondences: pair p's candidates are rows [offset[p], offset[p+1]) of rows[M,2] (offset
- *   nondecreasing from 0 to M, as the count writes it; any other table gives an unspecified but in-bounds sample),
+ *   nondecreasing within [0, M]; it may start above 0 and end below M, as a slice of a larger table does, and rows
+ *   outside [offset[0], offset[P]) belong to no pair; any other table gives an unspecified but in-bounds sample),
  *   n = their number. valid[p] = n >= max(min_count, 1), and without replacement n >= k. replace = 1: draw m is
  *   ((z >> 32) * n) >> 32 of its counter; replace = 0: the k candidates with the smallest (32-bit key, candidate), in
  *   that order. anc[P,k] = the anchor row, pos[P,k] = the positive row + anchor_len[p] (device int32 [P]), -1 for an
