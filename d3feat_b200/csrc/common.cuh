@@ -40,20 +40,20 @@ constexpr int kMaxBatch = 1024;
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 __host__ __device__ static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
-// Bump allocator over the caller-supplied workspace.
+// Bump allocator over a workspace: every buffer starts at a multiple of 256 bytes, and `off` ends at the bytes the
+// takes need. Each workspace has one layout function that runs the same takes to size it (null base: every pointer
+// is null) and to carve it.
 struct Carver {
   char* base;
-  size_t off;
-  size_t cap;
-  Carver(void* p, size_t bytes) : base((char*)p), off(0), cap(bytes) {}
+  size_t off = 0;
+  explicit Carver(void* p) : base((char*)p) {}
   template <typename T>
   T* take(size_t n) {
     off = align_up(off, 256);
-    T* r = (T*)(base + off);
+    T* r = base != nullptr ? (T*)(base + off) : nullptr;
     off += n * sizeof(T);
     return r;
   }
-  bool ok() const { return off <= cap; }
 };
 
 // ---- device helpers -------------------------------------------------------------------------------

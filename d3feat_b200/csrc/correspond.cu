@@ -297,7 +297,7 @@ size_t corr_layout(int N, int B, int P, double distance, const float* host_bbox,
   if (!corr_args_ok(N, B, P, distance, host_bbox)) return 0;
   const size_t nb = d3f_radius_neighbors_workspace_bytes(N, B, grid_radius(distance), host_bbox);
   if (nb == 0) return 0;
-  Carver cv(base, ~(size_t)0);
+  Carver cv(base);
   CorrWork x;
   x.start = cv.take<int>(B + 1);
   x.max_blocks = cv.take<int>(1);
@@ -404,7 +404,7 @@ int sort_bits(int P) {
 
 size_t sample_layout(int M, int P, SortBuffers* sb, void* base) {
   if (M < 0 || P < 1 || P > kMaxPairs) return 0;
-  Carver cv(base, ~(size_t)0);
+  Carver cv(base);
   SortBuffers s;
   for (int i = 0; i < 2; ++i) {
     s.keys[i] = cv.take<uint64_t>((size_t)std::max(M, 1));
@@ -520,7 +520,7 @@ aug_points_kernel(const float* __restrict__ points, const int4* __restrict__ inf
 
 size_t aug_layout(int B, int P, int** start, int4** info, void* base) {
   if (B < 1 || B > kMaxBatch || P < 1 || P > kMaxPairs) return 0;
-  Carver cv(base, ~(size_t)0);
+  Carver cv(base);
   int* s = cv.take<int>(B + 1);
   int4* i = cv.take<int4>(P);
   if (start != nullptr) *start = s;

@@ -328,15 +328,21 @@ eval_totals_kernel(int P, const __grid_constant__ EvalParams prm, Outputs o) {
 
 bool finite_positive(double x) { return std::isfinite(x) && x > 0.0; }
 
+// one int per pair and pose set (at least one set)
+size_t eval_layout(int P, int S, void* base, int** scratch) {
+  if (P < 1 || S < 0 || S > kMaxPoseSets) return 0;
+  Carver cv(base);
+  int* s = cv.take<int>((size_t)(S > 0 ? S : 1) * P);
+  if (scratch != nullptr) *scratch = s;
+  return cv.off;
+}
+
 }  // namespace
 }  // namespace d3f
 
 using namespace d3f;
 
-extern "C" size_t d3f_evaluate_pairs_workspace_bytes(int P, int S) {
-  if (P < 1 || S < 0 || S > kMaxPoseSets) return 0;
-  return align_up(sizeof(int) * (size_t)(S > 0 ? S : 1) * P, 256);
-}
+extern "C" size_t d3f_evaluate_pairs_workspace_bytes(int P, int S) { return eval_layout(P, S, nullptr, nullptr); }
 
 extern "C" int d3f_evaluate_pairs(const float* points, const int* count, int B, int k, const int* matches,
                                   const int* n_matches, int L, const int* pairs, int P, const double* truth_pose,
@@ -376,9 +382,10 @@ extern "C" int d3f_evaluate_pairs(const float* points, const int* count, int B, 
               D3F_ERR_INVALID, "evaluate_pairs: null pointer");
   for (int s = 0; s < S; ++s)
     D3F_REQUIRE(poses[s] != nullptr, D3F_ERR_INVALID, "evaluate_pairs: null pointer (poses[%d])", s);
-  D3F_REQUIRE(workspace_bytes >= d3f_evaluate_pairs_workspace_bytes(P, S), D3F_ERR_WORKSPACE,
-              "evaluate_pairs: workspace too small (%zu < %zu bytes)", workspace_bytes,
-              d3f_evaluate_pairs_workspace_bytes(P, S));
+  int* scratch;
+  const size_t need = eval_layout(P, S, workspace, &scratch);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE,
+              "evaluate_pairs: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
   EvalParams prm = {};
   for (int r = 0; r < R; ++r) prm.levels[r] = levels[r];
   prm.R = R;
@@ -391,7 +398,7 @@ extern "C" int d3f_evaluate_pairs(const float* points, const int* count, int B, 
   prm.rte_max = rte_max;
   prm.cos_max = std::cos(rre_max_deg * (3.141592653589793 / 180.0));   // the oracle's math.cos(deg * (pi / 180))
   Outputs o = {valid, n_match_inliers, inlier_ratio, fmr_hit, n_repeated, repeatability, rte, rre_deg, rmse2,
-               success, recall_hit, totals, (int*)workspace};
+               success, recall_hit, totals, scratch};
   eval_match_kernel<<<ceil_div(P, kPairWarps), kPairWarps * 32, 0, stream>>>(
       points, count, B, k, matches, n_matches, L, pairs, truth_flags, truth_pose, P, R, prm.tau_fmr2, fmr_ratio, o);
   D3F_LAUNCH_CHECK("eval_match_kernel");

@@ -272,8 +272,10 @@ struct SubsampleWs {
   int* n_rows;   // rows that belong to a cloud: min(row count, start[B]), written by bbox_batch_kernel
 };
 
-static size_t carve_subsample(Carver& cv, int N, int B, SubsampleWs& w) {
+static size_t subsample_layout(int N, int B, void* base, SubsampleWs* w_out) {
   int n = N > 0 ? N : 1;
+  Carver cv(base);
+  SubsampleWs w;
   w.sort.keys[0] = cv.take<uint64_t>(n);
   w.sort.keys[1] = cv.take<uint64_t>(n);
   w.sort.vals[0] = cv.take<uint32_t>(n);
@@ -288,6 +290,7 @@ static size_t carve_subsample(Carver& cv, int N, int B, SubsampleWs& w) {
   w.cell_count = cv.take<int>(n);
   w.err = cv.take<int>(1);
   w.n_rows = cv.take<int>(1);
+  if (w_out != nullptr) *w_out = w;
   return cv.off;
 }
 
@@ -301,11 +304,9 @@ int grid_subsample(const float* pts, const int* batch_len, int B, int N, float d
   D3F_REQUIRE(host_bbox != nullptr, D3F_ERR_INVALID, "grid_subsample: host_bbox is required");
   D3F_REQUIRE((feats == nullptr) == (fdim == 0) && (classes == nullptr) == (ldim == 0), D3F_ERR_INVALID,
               "grid_subsample: feats/fdim or classes/ldim mismatch");
-  D3F_REQUIRE(workspace_bytes >= d3f_grid_subsample_workspace_bytes(N, B), D3F_ERR_WORKSPACE,
-              "grid_subsample: workspace too small");
-  Carver cv(workspace, workspace_bytes);
   SubsampleWs w;
-  carve_subsample(cv, N, B, w);
+  const size_t need = subsample_layout(N, B, workspace, &w);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "grid_subsample: workspace too small");
 
   D3F_CUDA(cudaMemsetAsync(out_batch_len, 0, sizeof(int) * B, stream));
   D3F_CUDA(cudaMemsetAsync(out_M, 0, sizeof(int), stream));
@@ -357,20 +358,15 @@ int grid_subsample(const float* pts, const int* batch_len, int B, int N, float d
 }
 
 int grid_subsample_error_flag(const void* workspace, size_t workspace_bytes, int N, int B, int** flag) {
-  Carver cv(const_cast<void*>(workspace), workspace_bytes);
   SubsampleWs w;
-  carve_subsample(cv, N, B, w);
+  subsample_layout(N, B, const_cast<void*>(workspace), &w);
   *flag = w.err;
   return 0;
 }
 
 }  // namespace d3f
 
-extern "C" size_t d3f_grid_subsample_workspace_bytes(int N, int B) {
-  Carver cv(nullptr, ~(size_t)0);
-  SubsampleWs w;
-  return carve_subsample(cv, N, B, w) + 256;
-}
+extern "C" size_t d3f_grid_subsample_workspace_bytes(int N, int B) { return subsample_layout(N, B, nullptr, nullptr); }
 
 extern "C" int d3f_grid_subsample(const float* pts, const int* batch_len, int B, int N, float dl, const float* feats,
                                   int fdim, const int* classes, int ldim, const float* host_bbox, float* out_pts,

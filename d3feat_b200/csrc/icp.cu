@@ -319,7 +319,7 @@ size_t workspace_layout(int N, int B, int P, double distance, const float* host_
   if (g.ncells * B > kMaxGridCells || !nearest_lookup_exact(g, host_bbox)) return 0;
   const size_t nb = d3f_radius_neighbors_workspace_bytes(N, B, r, host_bbox);
   if (nb == 0) return 0;
-  Carver cv(base, ~(size_t)0);
+  Carver cv(base);
   Work x;
   x.start = cv.take<int>(B + 1);
   x.max_blocks = cv.take<int>(1);

@@ -108,15 +108,34 @@ static int keypoint_key_bits(int B) {
   return 32 + bits;
 }
 
+static size_t select_layout(int N, int B, void* base, int** start, SortBuffers* sb) {
+  if (N < 0 || B < 1) return 0;
+  Carver cv(base);
+  int* s = cv.take<int>((size_t)B + 1);
+  SortBuffers x;
+  x.keys[0] = cv.take<uint64_t>(N);
+  x.keys[1] = cv.take<uint64_t>(N);
+  x.vals[0] = cv.take<uint32_t>(N);
+  x.vals[1] = cv.take<uint32_t>(N);
+  x.block_hist = cv.take<int>(256 * (size_t)sort_num_blocks(N));
+  if (start != nullptr) *start = s;
+  if (sb != nullptr) *sb = x;
+  return cv.off;
+}
+
+static size_t sample_layout(int B, void* base, int** start) {
+  if (B < 1) return 0;
+  Carver cv(base);
+  int* s = cv.take<int>((size_t)B + 1);
+  if (start != nullptr) *start = s;
+  return cv.off;
+}
+
 }  // namespace d3f
 
 using namespace d3f;
 
-extern "C" size_t d3f_select_keypoints_workspace_bytes(int N, int B) {
-  if (N < 0 || B < 1) return 0;
-  return align_up(sizeof(int) * ((size_t)B + 1), 256) + 2 * align_up(sizeof(uint64_t) * (size_t)N, 256) +
-         2 * align_up(sizeof(uint32_t) * (size_t)N, 256) + align_up(sizeof(int) * 256 * (size_t)sort_num_blocks(N), 256);
-}
+extern "C" size_t d3f_select_keypoints_workspace_bytes(int N, int B) { return select_layout(N, B, nullptr, nullptr, nullptr); }
 
 extern "C" int d3f_select_keypoints(const float* scores, const int* lengths, int B, int N, int k, const float* points,
                                     const float* descriptors, int D, int* out_order, int* out_index, int* out_count,
@@ -135,16 +154,10 @@ extern "C" int d3f_select_keypoints(const float* scores, const int* lengths, int
               "select_keypoints: gathered descriptors requested without descriptors");
   D3F_REQUIRE(lengths != nullptr && workspace != nullptr && (scores != nullptr || N == 0), D3F_ERR_INVALID,
               "select_keypoints: null pointer");
-  D3F_REQUIRE(workspace_bytes >= d3f_select_keypoints_workspace_bytes(N, B), D3F_ERR_WORKSPACE,
-              "select_keypoints: workspace too small");
-  Carver cv(workspace, workspace_bytes);
-  int* start = cv.take<int>((size_t)B + 1);
+  int* start;
   SortBuffers sb;
-  sb.keys[0] = cv.take<uint64_t>(N);
-  sb.keys[1] = cv.take<uint64_t>(N);
-  sb.vals[0] = cv.take<uint32_t>(N);
-  sb.vals[1] = cv.take<uint32_t>(N);
-  sb.block_hist = cv.take<int>(256 * (size_t)sort_num_blocks(N));
+  const size_t need = select_layout(N, B, workspace, &start, &sb);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "select_keypoints: workspace too small");
   int rc = launch_batch_start(lengths, B, start, stream);
   if (rc) return rc;
   int cur = 0;
@@ -169,10 +182,7 @@ extern "C" int d3f_select_keypoints(const float* scores, const int* lengths, int
   return D3F_OK;
 }
 
-extern "C" size_t d3f_sample_keypoints_workspace_bytes(int B) {
-  if (B < 1) return 0;
-  return align_up(sizeof(int) * ((size_t)B + 1), 256);
-}
+extern "C" size_t d3f_sample_keypoints_workspace_bytes(int B) { return sample_layout(B, nullptr, nullptr); }
 
 extern "C" int d3f_sample_keypoints(const int* lengths, int B, int N, int k, uint64_t seed, const float* points,
                                     const float* descriptors, int D, const float* scores, int* out_index,
@@ -193,10 +203,9 @@ extern "C" int d3f_sample_keypoints(const int* lengths, int B, int N, int k, uin
   D3F_REQUIRE(out_scores == nullptr || scores != nullptr, D3F_ERR_INVALID,
               "sample_keypoints: gathered scores requested without scores");
   D3F_REQUIRE(lengths != nullptr && workspace != nullptr, D3F_ERR_INVALID, "sample_keypoints: null pointer");
-  D3F_REQUIRE(workspace_bytes >= d3f_sample_keypoints_workspace_bytes(B), D3F_ERR_WORKSPACE,
-              "sample_keypoints: workspace too small");
-  Carver cv(workspace, workspace_bytes);
-  int* start = cv.take<int>((size_t)B + 1);
+  int* start;
+  const size_t need = sample_layout(B, workspace, &start);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "sample_keypoints: workspace too small");
   int rc = launch_batch_start(lengths, B, start, stream);
   if (rc) return rc;
   const long long slots = (long long)B * k;

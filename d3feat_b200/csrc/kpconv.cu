@@ -1196,6 +1196,29 @@ int kpconv_stage1_wf(const float* q, const float4* s4, const int* idx, const flo
   return launch_stage1<false>(K, p, stream);
 }
 
+struct KpconvWs {
+  float* wf[2];   // stage 1 output, double-buffered (stage 1 of chunk i + 1 overlaps the GEMM of chunk i)
+  float* nn[2];   // 1 / neighbour count of each row of wf
+  float4* s4;     // packed supports + the shadow point
+  float* split;   // split-K partials of the tensor-core GEMM (null when it needs none)
+  float* w_img;   // weight image of the fused kernel
+};
+
+static size_t kpconv_layout(int Nq, int Ns, int K, int Cin, int Cout, void* base, KpconvWs* w_out) {
+  int chunk = chunk_queries(K, Cin);
+  if (chunk > Nq) chunk = Nq > 0 ? Nq : 1;
+  Carver cv(base);
+  KpconvWs w;
+  for (int b = 0; b < 2; ++b) w.wf[b] = cv.take<float>((size_t)chunk * K * Cin);
+  for (int b = 0; b < 2; ++b) w.nn[b] = cv.take<float>(chunk);
+  w.s4 = cv.take<float4>((size_t)Ns + 1);
+  const size_t split_floats = tc_gemm_split_ws_floats(chunk, Cout, K * Cin);
+  w.split = split_floats ? cv.take<float>(split_floats) : nullptr;
+  w.w_img = cv.take<float>(kpconv_fused_image_floats());
+  if (w_out != nullptr) *w_out = w;
+  return cv.off;
+}
+
 int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* idx, const float* feat,
                         const float* Kp, const float* offsets, const float* modulations, const float* W,
                         const float* W_packed, const int* query_order, int Nq, int Ns, int H, int K, int Cin, int Cout,
@@ -1214,17 +1237,13 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
   D3F_REQUIRE(extent > 0.f, D3F_ERR_INVALID, "kpconv: KP_extent=%g", (double)extent);
   D3F_REQUIRE((bn_scale == nullptr) == (bn_shift == nullptr), D3F_ERR_INVALID, "kpconv: bn_scale/bn_shift mismatch");
   D3F_REQUIRE(!deform || offsets != nullptr || Nq == 0, D3F_ERR_INVALID, "kpconv_deform: offsets missing");
-  D3F_REQUIRE(workspace_bytes >= d3f_kpconv_workspace_bytes(Nq, Ns, H, K, Cin, Cout), D3F_ERR_WORKSPACE,
-              "kpconv: workspace too small");
+  KpconvWs w;
+  const size_t need = kpconv_layout(Nq, Ns, K, Cin, Cout, workspace, &w);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "kpconv: workspace too small");
   if (Nq == 0) return D3F_OK;
   int chunk = chunk_queries(K, Cin);
   if (chunk > Nq) chunk = Nq;
-  Carver cv(workspace, workspace_bytes);
-  float* wf_buf[2] = {cv.take<float>((size_t)chunk * K * Cin), cv.take<float>((size_t)chunk * K * Cin)};
-  float* nn_buf[2] = {cv.take<float>(chunk), cv.take<float>(chunk)};
-  float4* s4 = cv.take<float4>((size_t)Ns + 1);
-  size_t split_floats = tc_gemm_split_ws_floats(chunk, Cout, K * Cin);
-  float* split_ws = split_floats ? cv.take<float>(split_floats) : nullptr;
+  float4* s4 = w.s4;
   const bool norm = normalize != 0 && !deform;
   {
     const int rc = kpconv_prep_supports(deform, s, feat, Ns, ns_dev, K, Cin, normalize, s4, stream);
@@ -1256,8 +1275,7 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
   }
   if (!deform && W_packed != nullptr &&
       kpconv_fused_supported(Nq, H, K, Cin, Cout, influence, mode, feat, W, out, query_order)) {
-    float* w_img = cv.take<float>(kpconv_fused_workspace_bytes() / sizeof(float));
-    return kpconv_fused_forward(q, s4, idx, feat, Kp, W, w_img, Nq, Ns, H, Cout, extent, norm ? 1 : 0, bn_scale, bn_shift,
+    return kpconv_fused_forward(q, s4, idx, feat, Kp, W, w.w_img, Nq, Ns, H, Cout, extent, norm ? 1 : 0, bn_scale, bn_shift,
                                 bias, leaky_alpha, out, stream, nq_dev, ns_dev);
   }
   Stage1Params p;
@@ -1281,8 +1299,8 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
   AuxStream* aux = n_chunks > 1 ? aux_stream() : nullptr;
   for (int ci = 0, n0 = 0; n0 < Nq; n0 += chunk, ++ci) {
     const int b = ci & 1;
-    float* wf = wf_buf[b];
-    float* inv_nn = nn_buf[b];
+    float* wf = w.wf[b];
+    float* inv_nn = w.nn[b];
     p.wf = wf;
     p.inv_nn = norm ? inv_nn : nullptr;
     p.n0 = n0;
@@ -1305,7 +1323,7 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
     ep.m_dev = nq_dev; ep.m_off = n0;                 // rows of this chunk that exist: clamp(*nq_dev - n0, 0, chunk)
     float* cbase = query_order ? out : out + (size_t)n0 * Cout;
     if (W_packed != nullptr && tc_gemm_supported(wf, K * Cin))
-      rc = tc_gemm(wf, W_packed, cbase, p.n1 - n0, Cout, K * Cin, ep, gs, split_ws);   // chunk GEMMs are serial on gs
+      rc = tc_gemm(wf, W_packed, cbase, p.n1 - n0, Cout, K * Cin, ep, gs, w.split);   // chunk GEMMs are serial on gs
     else
       rc = gemm_f32(wf, W, cbase, p.n1 - n0, Cout, K * Cin, ep, gs);
     if (rc) return rc;
@@ -1323,16 +1341,8 @@ int kpconv_forward_impl(bool deform, const float* q, const float* s, const int* 
 using namespace d3f;
 
 extern "C" size_t d3f_kpconv_workspace_bytes(int Nq, int Ns, int H, int K, int Cin, int Cout) {
-  (void)H; (void)Cout;
-  int chunk = chunk_queries(K, Cin);
-  if (chunk > Nq) chunk = Nq > 0 ? Nq : 1;
-  size_t b = 0;
-  b += 2 * align_up((size_t)chunk * K * Cin * sizeof(float), 256);   // wf is double-buffered (stage 1 / GEMM overlap)
-  b += 2 * align_up((size_t)chunk * sizeof(float), 256);
-  b += align_up((size_t)(Ns + 1) * sizeof(float4), 256);
-  b += align_up(tc_gemm_split_ws_floats(chunk, Cout, K * Cin) * sizeof(float), 256);
-  b += align_up(kpconv_fused_workspace_bytes(), 256);
-  return b + 1024;
+  (void)H;
+  return kpconv_layout(Nq, Ns, K, Cin, Cout, nullptr, nullptr);
 }
 
 extern "C" int d3f_kpconv_forward(const float* q, const float* s, const int* idx, const float* feat, const float* Kp,

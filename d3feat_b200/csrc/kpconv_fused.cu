@@ -450,7 +450,7 @@ bool kpconv_fused_supported(int Nq, int H, int K, int Cin, int Cout, int influen
          (reinterpret_cast<uintptr_t>(feat) & 15) == 0 && out != nullptr;
 }
 
-size_t kpconv_fused_workspace_bytes() { return (size_t)kFKp * kFWStage + 256; }
+size_t kpconv_fused_image_floats() { return (size_t)kFKp * kFWStage / sizeof(float); }
 
 int kpconv_fused_forward(const float* q, const float4* s4, const int* idx, const float* feat, const float* Kp,
                          const float* W, float* w_img, int Nq, int Ns, int H, int Cout, float extent, int normalize,

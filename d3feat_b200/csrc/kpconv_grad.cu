@@ -241,59 +241,60 @@ static int launch_wgrad_reduce(const float* partial, int nblk, long long MN, flo
 }
 
 // ---- KPConv --------------------------------------------------------------------------------------------------------
-struct BackwardLayout {
+struct BackwardWs {
   // persistent
-  size_t s4, G, rev, nKp, WT, WTp;
-  // phase region (reused: reverse table build, then the transposed forward, then the weight gradient)
-  size_t region;
-  size_t counts, offs, scan, keys0, keys1, vals0, vals1, hist, width;   // inside region, table build
-  size_t fwd_bytes;                                                    // inside region, transposed forward
-  size_t wf, partial;                                                  // inside region, weight gradient
-  size_t total;
+  float4* s4;
+  float *G, *nKp, *WT, *WTp;
+  int* rev;
+  // one region, reused by the reverse table build, then the transposed forward, then the weight gradient
+  char* region;
+  int *counts, *offs, *scan, *width;   // table build
+  SortBuffers sb;
+  size_t width_end;                    // bytes up to the reverse width: all that d3f_kpconv_reverse_width uses
+  size_t fwd_bytes;                    // transposed forward: the forward's own layout over the region
+  float *wf, *partial;                 // weight gradient
   int chunk, bpc, n_chunks;
 };
 
-static BackwardLayout backward_layout(int Nq, int Ns, int H, int K, int Cin, int Cout, int Hr) {
-  BackwardLayout L;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { off = align_up(off, 256); size_t r = off; off += bytes; return r; };
-  L.s4 = take((size_t)(Ns + 1) * sizeof(float4));
-  L.G = take((size_t)Nq * Cout * sizeof(float));
-  L.rev = take((size_t)Ns * (Hr > 0 ? Hr : 1) * sizeof(int));
-  L.nKp = take((size_t)K * 3 * sizeof(float));
-  L.WT = take((size_t)K * Cout * Cin * sizeof(float));
-  L.WTp = take(d3f_packed_weight_floats(K * Cout, Cin) * sizeof(float));
-  L.region = align_up(off, 256);
+// Persistent buffers first, then the region: each phase is measured with its own Carver over the region's base and
+// the region is as large as the largest phase.
+static size_t backward_layout(int Nq, int Ns, int H, int K, int Cin, int Cout, int Hr, void* base, BackwardWs* w_out) {
+  if (Nq < 0 || Ns < 0 || H < 0 || K < 1 || Cin < 1 || Cout < 1 || Hr < 0) return 0;
+  Carver cv(base);
+  BackwardWs w;
+  w.s4 = cv.take<float4>((size_t)Ns + 1);
+  w.G = cv.take<float>((size_t)Nq * Cout);
+  w.rev = cv.take<int>((size_t)Ns * (Hr > 0 ? Hr : 1));
+  w.nKp = cv.take<float>((size_t)K * 3);
+  w.WT = cv.take<float>((size_t)K * Cout * Cin);
+  w.WTp = cv.take<float>(d3f_packed_weight_floats(K * Cout, Cin));
+  w.region = cv.take<char>(0);
+  const size_t region_off = cv.off;
   // table build
   const long long E = (long long)Nq * H;
-  size_t r = 0;
-  auto rtake = [&](size_t bytes) { r = align_up(r, 256); size_t o = r; r += bytes; return o; };
-  L.counts = rtake((size_t)(Ns + 1) * sizeof(int));
-  L.offs = rtake((size_t)(Ns + 1) * sizeof(int));
-  L.scan = rtake((size_t)(scan_num_blocks(Ns + 1) + 1) * sizeof(int));
-  L.width = rtake(sizeof(int));
-  L.keys0 = rtake((size_t)E * sizeof(uint64_t));
-  L.keys1 = rtake((size_t)E * sizeof(uint64_t));
-  L.vals0 = rtake((size_t)E * sizeof(uint32_t));
-  L.vals1 = rtake((size_t)E * sizeof(uint32_t));
-  L.hist = rtake((size_t)256 * sort_num_blocks((int)E) * sizeof(int));
-  const size_t build = align_up(r, 256);
+  Carver build(w.region);
+  w.counts = build.take<int>((size_t)Ns + 1);
+  w.offs = build.take<int>((size_t)Ns + 1);
+  w.scan = build.take<int>((size_t)scan_num_blocks(Ns + 1) + 1);
+  w.width = build.take<int>(1);
+  w.width_end = region_off + build.off;
+  w.sb.keys[0] = build.take<uint64_t>(E);
+  w.sb.keys[1] = build.take<uint64_t>(E);
+  w.sb.vals[0] = build.take<uint32_t>(E);
+  w.sb.vals[1] = build.take<uint32_t>(E);
+  w.sb.block_hist = build.take<int>((size_t)256 * sort_num_blocks((int)E));
   // transposed forward: Ns queries, Nq supports, Hr neighbours, Cout -> Cin channels
-  L.fwd_bytes = d3f_kpconv_workspace_bytes(Ns, Nq, Hr, K, Cout, Cin);
+  w.fwd_bytes = d3f_kpconv_workspace_bytes(Ns, Nq, Hr, K, Cout, Cin);
   // weight gradient
-  L.chunk = kpconv_chunk_queries(K, Cin);
-  if (L.chunk > Nq) L.chunk = Nq > 0 ? Nq : 1;
-  L.n_chunks = Nq > 0 ? ceil_div(Nq, L.chunk) : 0;
-  L.bpc = wgrad_blocks(L.chunk);
-  r = 0;
-  L.wf = rtake((size_t)L.chunk * K * Cin * sizeof(float));
-  L.partial = rtake((size_t)(L.n_chunks > 0 ? L.n_chunks : 1) * L.bpc * K * Cin * Cout * sizeof(float));
-  const size_t wgrad = align_up(r, 256);
-  size_t region = build;
-  if (L.fwd_bytes > region) region = L.fwd_bytes;
-  if (wgrad > region) region = wgrad;
-  L.total = L.region + region + 1024;
-  return L;
+  w.chunk = kpconv_chunk_queries(K, Cin);
+  if (w.chunk > Nq) w.chunk = Nq > 0 ? Nq : 1;
+  w.n_chunks = Nq > 0 ? ceil_div(Nq, w.chunk) : 0;
+  w.bpc = wgrad_blocks(w.chunk);
+  Carver wgrad(w.region);
+  w.wf = wgrad.take<float>((size_t)w.chunk * K * Cin);
+  w.partial = wgrad.take<float>((size_t)(w.n_chunks > 0 ? w.n_chunks : 1) * w.bpc * K * Cin * Cout);
+  if (w_out != nullptr) *w_out = w;
+  return region_off + std::max(std::max(build.off, w.fwd_bytes), wgrad.off);
 }
 
 }  // namespace d3f
@@ -301,8 +302,7 @@ static BackwardLayout backward_layout(int Nq, int Ns, int H, int K, int Cin, int
 using namespace d3f;
 
 extern "C" size_t d3f_kpconv_backward_workspace_bytes(int Nq, int Ns, int H, int K, int Cin, int Cout, int Hr) {
-  if (Nq < 0 || Ns < 0 || H < 0 || K < 1 || Cin < 1 || Cout < 1 || Hr < 0) return 0;
-  return backward_layout(Nq, Ns, H, K, Cin, Cout, Hr).total;
+  return backward_layout(Nq, Ns, H, K, Cin, Cout, Hr, nullptr, nullptr);
 }
 
 extern "C" int d3f_kpconv_reverse_width(const int* idx, int Nq, int Ns, int H, int* width, void* workspace,
@@ -314,19 +314,17 @@ extern "C" int d3f_kpconv_reverse_width(const int* idx, int Nq, int Ns, int H, i
   *width = 0;
   if (Nq == 0 || Ns == 0 || H == 0) return D3F_OK;
   D3F_REQUIRE(idx != nullptr && workspace != nullptr, D3F_ERR_INVALID, "kpconv_reverse_width: null pointer");
-  const BackwardLayout L = backward_layout(Nq, Ns, H, 1, 1, 1, 0);
-  D3F_REQUIRE(workspace_bytes >= L.region + L.width + sizeof(int), D3F_ERR_WORKSPACE,
-              "kpconv_reverse_width: workspace too small");
-  char* reg = static_cast<char*>(workspace) + L.region;
-  int* counts = reinterpret_cast<int*>(reg + L.counts);
-  int* dwidth = reinterpret_cast<int*>(reg + L.width);
-  D3F_CUDA(cudaMemsetAsync(counts, 0, (size_t)Ns * sizeof(int), stream));
+  // the smallest backward layout of these rows: any workspace of d3f_kpconv_backward_workspace_bytes(..., Hr = 0) holds it
+  BackwardWs w;
+  backward_layout(Nq, Ns, H, 1, 1, 1, 0, workspace, &w);
+  D3F_REQUIRE(workspace_bytes >= w.width_end, D3F_ERR_WORKSPACE, "kpconv_reverse_width: workspace too small");
+  D3F_CUDA(cudaMemsetAsync(w.counts, 0, (size_t)Ns * sizeof(int), stream));
   reverse_keys_kernel<<<grid_for((long long)Nq * H), 256, 0, stream>>>(idx, Nq, Ns, H, nq_dev, ns_dev, nullptr, nullptr,
-                                                                       counts);
+                                                                       w.counts);
   D3F_LAUNCH_CHECK("reverse_keys_kernel");
-  max_count_kernel<<<1, 1024, 0, stream>>>(counts, Ns, dwidth);
+  max_count_kernel<<<1, 1024, 0, stream>>>(w.counts, Ns, w.width);
   D3F_LAUNCH_CHECK("max_count_kernel");
-  D3F_CUDA(cudaMemcpyAsync(width, dwidth, sizeof(int), cudaMemcpyDeviceToHost, stream));
+  D3F_CUDA(cudaMemcpyAsync(width, w.width, sizeof(int), cudaMemcpyDeviceToHost, stream));
   D3F_CUDA(cudaStreamSynchronize(stream));
   return D3F_OK;
 }
@@ -350,16 +348,15 @@ extern "C" int d3f_kpconv_backward(const float* q, const float* s, const int* id
   D3F_REQUIRE(extent > 0.f, D3F_ERR_INVALID, "kpconv_backward: KP_extent=%g", (double)extent);
   D3F_REQUIRE((long long)Nq * H < (1ll << 31), D3F_ERR_INVALID, "kpconv_backward: Nq*H=%lld beyond int32",
               (long long)Nq * H);
-  const BackwardLayout L = backward_layout(Nq, Ns, H, K, Cin, Cout, Hr);
-  D3F_REQUIRE(workspace_bytes >= L.total, D3F_ERR_WORKSPACE, "kpconv_backward: workspace too small");
+  BackwardWs w;
+  const size_t need = backward_layout(Nq, Ns, H, K, Cin, Cout, Hr, workspace, &w);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "kpconv_backward: workspace too small");
   if (dfeat != nullptr && Ns > 0) D3F_CUDA(cudaMemsetAsync(dfeat, 0, (size_t)Ns * Cin * sizeof(float), stream));
   if (dW != nullptr) D3F_CUDA(cudaMemsetAsync(dW, 0, (size_t)K * Cin * Cout * sizeof(float), stream));
   if (Nq == 0 || Ns == 0 || (dfeat == nullptr && dW == nullptr)) return D3F_OK;
 
-  char* ws = static_cast<char*>(workspace);
-  char* reg = ws + L.region;
-  float4* s4 = reinterpret_cast<float4*>(ws + L.s4);
-  float* G = reinterpret_cast<float*>(ws + L.G);
+  float4* s4 = w.s4;
+  float* G = w.G;
   int rc = kpconv_prep_supports(false, s, feat, Ns, ns_dev, K, Cin, normalize, s4, stream);
   if (rc) return rc;
   grad_rowscale_kernel<<<ceil_div(Nq * 32, 256), 256, 0, stream>>>(dout, idx, s4, Nq, Ns, H, Cout, normalize != 0,
@@ -367,66 +364,64 @@ extern "C" int d3f_kpconv_backward(const float* q, const float* s, const int* id
   D3F_LAUNCH_CHECK("grad_rowscale_kernel");
 
   if (dfeat != nullptr && Hr > 0 && H > 0) {
-    int* counts = reinterpret_cast<int*>(reg + L.counts);
-    int* offs = reinterpret_cast<int*>(reg + L.offs);
-    int* rev = reinterpret_cast<int*>(ws + L.rev);
-    SortBuffers sb;
-    sb.keys[0] = reinterpret_cast<uint64_t*>(reg + L.keys0);
-    sb.keys[1] = reinterpret_cast<uint64_t*>(reg + L.keys1);
-    sb.vals[0] = reinterpret_cast<uint32_t*>(reg + L.vals0);
-    sb.vals[1] = reinterpret_cast<uint32_t*>(reg + L.vals1);
-    sb.block_hist = reinterpret_cast<int*>(reg + L.hist);
     const uint32_t* sorted_q = nullptr;
-    rc = reverse_csr(idx, Nq, Ns, H, nq_dev, ns_dev, sb, counts, offs, reinterpret_cast<int*>(reg + L.scan), &sorted_q,
-                     stream);
+    rc = reverse_csr(idx, Nq, Ns, H, nq_dev, ns_dev, w.sb, w.counts, w.offs, w.scan, &sorted_q, stream);
     if (rc) return rc;
-    reverse_fill_kernel<<<grid_for((long long)Ns * Hr), 256, 0, stream>>>(counts, offs, sorted_q, Ns, Hr, Nq, rev);
+    reverse_fill_kernel<<<grid_for((long long)Ns * Hr), 256, 0, stream>>>(w.counts, w.offs, sorted_q, Ns, Hr, Nq,
+                                                                          w.rev);
     D3F_LAUNCH_CHECK("reverse_fill_kernel");
     // W^T [K, Cout, Cin] (packed for the tensor-core contraction), -Kp
-    float* WT = reinterpret_cast<float*>(ws + L.WT);
-    float* nKp = reinterpret_cast<float*>(ws + L.nKp);
-    transpose_weights_kernel<<<grid_for((long long)K * Cin * Cout), 256, 0, stream>>>(W, K, Cin, Cout, WT);
+    transpose_weights_kernel<<<grid_for((long long)K * Cin * Cout), 256, 0, stream>>>(W, K, Cin, Cout, w.WT);
     D3F_LAUNCH_CHECK("transpose_weights_kernel");
-    negate_kernel<<<1, 256, 0, stream>>>(Kp, K * 3, nKp);
+    negate_kernel<<<1, 256, 0, stream>>>(Kp, K * 3, w.nKp);
     D3F_LAUNCH_CHECK("negate_kernel");
     float* WTp = nullptr;
     if (tensor_cores) {
-      WTp = reinterpret_cast<float*>(ws + L.WTp);
-      rc = d3f_pack_weight(WT, K * Cout, Cin, WTp, stream);
+      WTp = w.WTp;
+      rc = d3f_pack_weight(w.WT, K * Cout, Cin, WTp, stream);
       if (rc) return rc;
     }
-    rc = kpconv_forward_impl(false, s, q, rev, G, nKp, nullptr, nullptr, WT, WTp, nullptr, Ns, Nq, Hr, K, Cout, Cin,
-                             extent, influence, mode, 0, nullptr, nullptr, nullptr, -1.f, dfeat, reg, L.fwd_bytes,
-                             stream, ns_dev, nq_dev);
+    rc = kpconv_forward_impl(false, s, q, w.rev, G, w.nKp, nullptr, nullptr, w.WT, WTp, nullptr, Ns, Nq, Hr, K, Cout,
+                             Cin, extent, influence, mode, 0, nullptr, nullptr, nullptr, -1.f, dfeat, w.region,
+                             w.fwd_bytes, stream, ns_dev, nq_dev);
     if (rc) return rc;
   }
 
   if (dW != nullptr) {
-    float* wf = reinterpret_cast<float*>(reg + L.wf);
-    float* partial = reinterpret_cast<float*>(reg + L.partial);
     const int M = K * Cin;
-    for (int ci = 0, n0 = 0; n0 < Nq; n0 += L.chunk, ++ci) {
-      const int n1 = min(Nq, n0 + L.chunk);
-      rc = kpconv_stage1_wf(q, s4, idx, feat, Kp, Nq, Ns, H, K, Cin, extent, influence, mode, n0, n1, wf, stream,
+    for (int ci = 0, n0 = 0; n0 < Nq; n0 += w.chunk, ++ci) {
+      const int n1 = min(Nq, n0 + w.chunk);
+      rc = kpconv_stage1_wf(q, s4, idx, feat, Kp, Nq, Ns, H, K, Cin, extent, influence, mode, n0, n1, w.wf, stream,
                             nq_dev, ns_dev);
       if (rc) return rc;
-      rc = launch_wgrad_partial(wf, G + (size_t)n0 * Cout, n1 - n0, M, Cout, nq_dev, n0, L.bpc,
-                                partial + (size_t)ci * L.bpc * M * Cout, stream);
+      rc = launch_wgrad_partial(w.wf, G + (size_t)n0 * Cout, n1 - n0, M, Cout, nq_dev, n0, w.bpc,
+                                w.partial + (size_t)ci * w.bpc * M * Cout, stream);
       if (rc) return rc;
     }
-    rc = launch_wgrad_reduce(partial, L.n_chunks * L.bpc, (long long)M * Cout, dW, stream);
+    rc = launch_wgrad_reduce(w.partial, w.n_chunks * w.bpc, (long long)M * Cout, dW, stream);
     if (rc) return rc;
   }
   return D3F_OK;
 }
 
 // ---- unary ----------------------------------------------------------------------------------------------------------
-extern "C" size_t d3f_unary_backward_workspace_bytes(int N, int Cin, int Cout) {
+struct UnaryBackwardWs {
+  float *WT, *WTp, *partial;
+};
+
+static size_t unary_backward_layout(int N, int Cin, int Cout, void* base, UnaryBackwardWs* w_out) {
   if (N < 0 || Cin < 1 || Cout < 1) return 0;
-  size_t b = align_up((size_t)Cin * Cout * sizeof(float), 256);
-  b += align_up(d3f_packed_weight_floats(Cout, Cin) * sizeof(float), 256);
-  b += align_up((size_t)wgrad_blocks(N) * Cin * Cout * sizeof(float), 256);
-  return b + 1024;
+  Carver cv(base);
+  UnaryBackwardWs w;
+  w.WT = cv.take<float>((size_t)Cin * Cout);
+  w.WTp = cv.take<float>(d3f_packed_weight_floats(Cout, Cin));
+  w.partial = cv.take<float>((size_t)wgrad_blocks(N) * Cin * Cout);
+  if (w_out != nullptr) *w_out = w;
+  return cv.off;
+}
+
+extern "C" size_t d3f_unary_backward_workspace_bytes(int N, int Cin, int Cout) {
+  return unary_backward_layout(N, Cin, Cout, nullptr, nullptr);
 }
 
 extern "C" int d3f_unary_backward(const float* x, const float* W, const float* dout, int N, int Cin, int Cout,
@@ -437,15 +432,13 @@ extern "C" int d3f_unary_backward(const float* x, const float* W, const float* d
               "d3f_unary_backward: null pointer");
   D3F_REQUIRE(N >= 0 && Cin >= 1 && Cout >= 1, D3F_ERR_INVALID, "unary_backward: bad shape N=%d Cin=%d Cout=%d", N,
               Cin, Cout);
-  D3F_REQUIRE(workspace_bytes >= d3f_unary_backward_workspace_bytes(N, Cin, Cout), D3F_ERR_WORKSPACE,
-              "unary_backward: workspace too small");
+  UnaryBackwardWs w;
+  const size_t need = unary_backward_layout(N, Cin, Cout, workspace, &w);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "unary_backward: workspace too small");
   if (dx != nullptr && N > 0) D3F_CUDA(cudaMemsetAsync(dx, 0, (size_t)N * Cin * sizeof(float), stream));
   if (dW != nullptr) D3F_CUDA(cudaMemsetAsync(dW, 0, (size_t)Cin * Cout * sizeof(float), stream));
   if (N == 0) return D3F_OK;
-  Carver cv(workspace, workspace_bytes);
-  float* WT = cv.take<float>((size_t)Cin * Cout);
-  float* WTp = cv.take<float>(d3f_packed_weight_floats(Cout, Cin));
-  float* partial = cv.take<float>((size_t)wgrad_blocks(N) * Cin * Cout);
+  float *WT = w.WT, *WTp = w.WTp, *partial = w.partial;
   int rc;
   if (dx != nullptr) {   // dx = dout @ W^T through the forward GEMM
     transpose_weights_kernel<<<grid_for((long long)Cin * Cout), 256, 0, stream>>>(W, 1, Cin, Cout, WT);

@@ -197,14 +197,24 @@ match_finalize_kernel(const int* __restrict__ count, int B, int k, const int* __
   }
 }
 
+// the best key of every row and every column of each pair's k x k similarity matrix
+size_t match_layout(int k, int P, void* base, unsigned long long** row_key, unsigned long long** col_key) {
+  if (k < 1 || P < 1 || (long long)P * k > INT32_MAX) return 0;
+  Carver cv(base);
+  unsigned long long* r = cv.take<unsigned long long>((size_t)P * k);
+  unsigned long long* c = cv.take<unsigned long long>((size_t)P * k);
+  if (row_key != nullptr) *row_key = r;
+  if (col_key != nullptr) *col_key = c;
+  return cv.off;
+}
+
 }  // namespace
 }  // namespace d3f
 
 using namespace d3f;
 
 extern "C" size_t d3f_match_descriptors_workspace_bytes(int k, int P) {
-  if (k < 1 || P < 1 || (long long)P * k > INT32_MAX) return 0;
-  return 2 * align_up(sizeof(unsigned long long) * (size_t)P * k, 256);
+  return match_layout(k, P, nullptr, nullptr, nullptr);
 }
 
 extern "C" int d3f_match_descriptors(const float* desc, const int* count, int B, int k, int D, const int* pairs, int P,
@@ -217,13 +227,11 @@ extern "C" int d3f_match_descriptors(const float* desc, const int* count, int B,
               (long long)P * k);
   D3F_REQUIRE(desc && count && pairs && nn_st && sim_st && nn_ts && sim_ts && matches && n_matches && workspace,
               D3F_ERR_INVALID, "match_descriptors: null pointer");
-  D3F_REQUIRE(workspace_bytes >= d3f_match_descriptors_workspace_bytes(k, P), D3F_ERR_WORKSPACE,
-              "match_descriptors: workspace too small");
-  Carver cv(workspace, workspace_bytes);
-  unsigned long long* row_key = cv.take<unsigned long long>((size_t)P * k);
-  unsigned long long* col_key = cv.take<unsigned long long>((size_t)P * k);
-  // key 0 is below every real key (score_ord is never 0): "no candidate yet"
-  D3F_CUDA(cudaMemsetAsync(workspace, 0, d3f_match_descriptors_workspace_bytes(k, P), stream));
+  unsigned long long *row_key, *col_key;
+  const size_t need = match_layout(k, P, workspace, &row_key, &col_key);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "match_descriptors: workspace too small");
+  // key 0 is below every real key (score_ord is never 0): "no candidate yet". One memset over both key arrays.
+  D3F_CUDA(cudaMemsetAsync(row_key, 0, need, stream));
   const int T = ceil_div(k, kTile);
   const long long tiles = (long long)P * T * T;
   const int blocks = (int)min(tiles, (long long)32 * kNumSMs);

@@ -66,8 +66,15 @@ struct NbWs {
   int* scan_scratch;
 };
 
-static size_t carve_nb(Carver& cv, int Ns, int B, long long total_cells, NbWs& w) {
+// The workspace of a grid over Ns supports at `radius`, or 0 for a grid the search refuses.
+static size_t nb_layout(int Ns, int B, float radius, const float* host_bbox, void* base, NbWs* w_out) {
+  if (host_bbox == nullptr || !(radius > 0.f) || B < 1) return 0;
+  const NbGrid g = make_grid(host_bbox, radius);
+  const long long total_cells = g.ncells * B;
+  if (total_cells > kMaxGridCells || !radius_scan_complete(g)) return 0;
   int n = Ns > 0 ? Ns : 1;
+  Carver cv(base);
+  NbWs w;
   w.cell_id = cv.take<uint32_t>(n);
   w.s_start = cv.take<int>(B + 1);
   w.q_start = cv.take<int>(B + 1);
@@ -75,6 +82,7 @@ static size_t carve_nb(Carver& cv, int Ns, int B, long long total_cells, NbWs& w
   w.cell_start = cv.take<int>((size_t)total_cells + 1);
   w.cell_cnt = cv.take<int>((size_t)total_cells + 1);
   w.scan_scratch = cv.take<int>((size_t)scan_num_blocks((int)total_cells) + 1);
+  if (w_out != nullptr) *w_out = w;
   return cv.off;
 }
 
@@ -92,11 +100,9 @@ int radius_neighbors_build(const float* supports, const int* s_batch_len, int B,
   D3F_REQUIRE(radius_scan_complete(g), D3F_ERR_INVALID,
               "radius_neighbors: grid %d x %d x %d has an axis longer than %d cells (of radius * 1.001)", g.nx, g.ny,
               g.nz, kMaxScanAxisCells);
-  D3F_REQUIRE(workspace_bytes >= d3f_radius_neighbors_workspace_bytes(Ns, B, radius, host_bbox), D3F_ERR_WORKSPACE,
-              "radius_neighbors: workspace too small");
-  Carver cv(workspace, workspace_bytes);
   NbWs w;
-  carve_nb(cv, Ns, B, total, w);
+  const size_t need = nb_layout(Ns, B, radius, host_bbox, workspace, &w);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "radius_neighbors: workspace too small");
   if (s_start_pre != nullptr) w.s_start = const_cast<int*>(s_start_pre);   // the caller already scanned these lengths
   else if (launch_batch_start(s_batch_len, B, w.s_start, stream)) return D3F_ERR_CUDA;
   D3F_CUDA(cudaMemsetAsync(w.cell_cnt, 0, sizeof(int) * ((size_t)total + 1), stream));
@@ -121,9 +127,10 @@ int radius_neighbors_view(const void* workspace, int Ns, int B, float radius, co
   NbGrid g = make_grid(host_bbox, radius);
   long long total = g.ncells * B;
   D3F_REQUIRE(total <= kMaxGridCells, D3F_ERR_CAPACITY, "radius_neighbors: grid too large");
-  Carver cv(const_cast<void*>(workspace), ~(size_t)0);
+  // as in d3f_radius_neighbors_order: no grid of these arguments can have been built
   NbWs w;
-  carve_nb(cv, Ns, B, total, w);
+  D3F_REQUIRE(nb_layout(Ns, B, radius, host_bbox, const_cast<void*>(workspace), &w) > 0, D3F_ERR_INVALID,
+              "radius_neighbors_view: no grid of these arguments can be built");
   out->g = g;
   out->sorted_pts = w.sorted_pts;
   out->cell_start = w.cell_start;
@@ -604,9 +611,8 @@ static int query_common(bool fill, const float* queries, const int* q_batch_len,
   D3F_REQUIRE(radius_scan_complete(g), D3F_ERR_INVALID,
               "radius_neighbors: grid %d x %d x %d has an axis longer than %d cells (of radius * 1.001)", g.nx, g.ny,
               g.nz, kMaxScanAxisCells);
-  Carver cv(const_cast<void*>(workspace), ~(size_t)0);
   NbWs w;
-  carve_nb(cv, Ns, B, total, w);
+  nb_layout(Ns, B, radius, host_bbox, const_cast<void*>(workspace), &w);
   if (q_start_pre != nullptr) w.q_start = const_cast<int*>(q_start_pre);
   else if (launch_batch_start(q_batch_len, B, w.q_start, stream)) return D3F_ERR_CUDA;
   if (out_max != nullptr && !fill) D3F_CUDA(cudaMemsetAsync(out_max, 0, sizeof(int), stream));
@@ -652,13 +658,7 @@ int radius_neighbors_fill(const float* queries, const int* q_batch_len, int Nq, 
 using namespace d3f;
 
 extern "C" size_t d3f_radius_neighbors_workspace_bytes(int Ns, int B, float radius, const float* host_bbox) {
-  if (host_bbox == nullptr || !(radius > 0.f) || B < 1) return 0;
-  NbGrid g = make_grid(host_bbox, radius);
-  long long total = g.ncells * B;
-  if (total > kMaxGridCells || !radius_scan_complete(g)) return 0;
-  Carver cv(nullptr, ~(size_t)0);
-  NbWs w;
-  return carve_nb(cv, Ns, B, total, w) + 256;
+  return nb_layout(Ns, B, radius, host_bbox, nullptr, nullptr);
 }
 
 extern "C" int d3f_radius_neighbors_build(const float* supports, const int* s_batch_len, int B, int Ns, float radius,
@@ -706,9 +706,10 @@ extern "C" int d3f_radius_neighbors_order(const void* workspace, int Ns, int B, 
   NbGrid g = make_grid(host_bbox, radius);
   long long total = g.ncells * B;
   D3F_REQUIRE(total <= kMaxGridCells, D3F_ERR_CAPACITY, "radius_neighbors: grid too large");
-  Carver cv(const_cast<void*>(workspace), ~(size_t)0);
+  // arguments whose grid d3f_radius_neighbors_build refuses have no workspace to order (the layout is 0)
   NbWs w;
-  carve_nb(cv, Ns, B, total, w);
+  D3F_REQUIRE(nb_layout(Ns, B, radius, host_bbox, const_cast<void*>(workspace), &w) > 0, D3F_ERR_INVALID,
+              "radius_neighbors_order: no grid of these arguments can be built");
   cell_order_kernel<<<ceil_div(Ns, 256), 256, 0, stream>>>(w.sorted_pts, Ns, out_order);
   D3F_LAUNCH_CHECK("cell_order_kernel");
   return D3F_OK;

@@ -75,7 +75,7 @@ int reverse_csr(const int* idx, int Nq, int Ns, int H, const int* nq_dev, const 
 // ---- kpconv_fused.cu (one persistent kernel per layer: gather + correlation + wgmma contraction) -------
 bool kpconv_fused_supported(int Nq, int H, int K, int Cin, int Cout, int influence, int mode, const float* feat,
                             const float* W, const float* out, const int* query_order);
-size_t kpconv_fused_workspace_bytes();
+size_t kpconv_fused_image_floats();
 int kpconv_fused_forward(const float* q, const float4* s4, const int* idx, const float* feat, const float* Kp,
                          const float* W, float* w_img, int Nq, int Ns, int H, int Cout, float extent, int normalize,
                          const float* bn_scale, const float* bn_shift, const float* bias, float leaky_alpha, float* out,

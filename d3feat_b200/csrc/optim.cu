@@ -230,13 +230,22 @@ static long long partial_capacity(int T, long long numel_total) {
   return (numel_total + kOptBlock - 1) / kOptBlock + T;   // every tensor ends at most one partial block early
 }
 
+// One fp64 partial per block of the table, up to partial_capacity; at least one, so that the query of an empty table
+// is not 0 (which means refused).
+static size_t momentum_layout(int T, long long numel_total, void* base, double** partial) {
+  if (T < 0 || T > kOptMaxTensors || numel_total < 0) return 0;
+  Carver cv(base);
+  double* p = cv.take<double>((size_t)max(partial_capacity(T, numel_total), 1ll));
+  if (partial != nullptr) *partial = p;
+  return cv.off;
+}
+
 }  // namespace d3f
 
 using namespace d3f;
 
 extern "C" size_t d3f_momentum_clip_workspace_bytes(int T, long long numel_total) {
-  if (T < 0 || T > kOptMaxTensors || numel_total < 0) return 0;
-  return align_up((size_t)partial_capacity(T, numel_total) * sizeof(double), 256) + 256;
+  return momentum_layout(T, numel_total, nullptr, nullptr);
 }
 
 extern "C" int d3f_momentum_clip_update(const d3f_momentum_tensor* table, int T, long long numel_total, float lr,
@@ -250,10 +259,10 @@ extern "C" int d3f_momentum_clip_update(const d3f_momentum_tensor* table, int T,
               (double)clip_norm);
   if (T == 0 || numel_total == 0) return D3F_OK;
   D3F_REQUIRE(table != nullptr && workspace != nullptr, D3F_ERR_INVALID, "momentum_clip_update: null pointer");
-  D3F_REQUIRE(workspace_bytes >= d3f_momentum_clip_workspace_bytes(T, numel_total), D3F_ERR_WORKSPACE,
-              "momentum_clip_update: workspace too small");
+  double* partial;
+  const size_t need = momentum_layout(T, numel_total, workspace, &partial);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "momentum_clip_update: workspace too small");
   const long long cap = partial_capacity(T, numel_total);
-  double* partial = (double*)workspace;
   if (clip_norm > 0.f) {
     const long long warps = (cap + 31) / 32;            // a warp per 32 blocks
     const long long per_cta = kPartialThreads / 32;

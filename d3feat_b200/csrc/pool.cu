@@ -95,11 +95,19 @@ ind_max_pool_fix_kernel(const int* __restrict__ inds, int N1cap, int N2cap, cons
   }
 }
 
+// [C] ordered column minima + [1] flag (0xFFFFFFFF = not needed)
+static size_t ind_max_pool_layout(int C, void* base, unsigned** colmin) {
+  Carver cv(base);
+  unsigned* c = cv.take<unsigned>((size_t)(C > 0 ? C : 1) + 1);
+  if (colmin != nullptr) *colmin = c;
+  return cv.off;
+}
+
 }  // namespace d3f
 
 using namespace d3f;
 
-extern "C" size_t d3f_ind_max_pool_workspace_bytes(int C) { return sizeof(unsigned) * ((size_t)(C > 0 ? C : 1) + 1); }
+extern "C" size_t d3f_ind_max_pool_workspace_bytes(int C) { return ind_max_pool_layout(C, nullptr, nullptr); }
 
 extern "C" int d3f_ind_max_pool(const float* x, const int* inds, int N1, int N2, int H, int C, float* out,
                                 void* workspace, size_t workspace_bytes, d3f_stream_t stream_, const int* n1_dev,
@@ -108,11 +116,11 @@ extern "C" int d3f_ind_max_pool(const float* x, const int* inds, int N1, int N2,
   D3F_REQUIRE(N2 == 0 || (x && inds && out && workspace), D3F_ERR_INVALID, "d3f_ind_max_pool: null pointer");
   D3F_REQUIRE(N1 >= 1 && N2 >= 0 && H >= 0 && C >= 1, D3F_ERR_INVALID, "ind_max_pool: bad shape N1=%d N2=%d H=%d C=%d",
               N1, N2, H, C);
-  D3F_REQUIRE(workspace_bytes >= sizeof(unsigned) * ((size_t)C + 1), D3F_ERR_WORKSPACE,
-              "ind_max_pool: workspace too small");
+  unsigned* colmin;
+  const size_t need = ind_max_pool_layout(C, workspace, &colmin);
+  D3F_REQUIRE(workspace_bytes >= need, D3F_ERR_WORKSPACE, "ind_max_pool: workspace too small");
   if (N2 == 0) return D3F_OK;
-  unsigned* colmin = (unsigned*)workspace;   // [C] ordered column minima + [1] flag (0xFFFFFFFF = not needed)
-  D3F_CUDA(cudaMemsetAsync(colmin, 0xff, sizeof(unsigned) * ((size_t)C + 1), stream));
+  D3F_CUDA(cudaMemsetAsync(colmin, 0xff, need, stream));
   int blocks = ceil_div(N2 * 32, 256);
   bool v4 = (C % 4 == 0) && ((reinterpret_cast<uintptr_t>(x) & 15) == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
   const int slabs = ceil_div(C, v4 ? 128 : 32);
@@ -262,11 +270,25 @@ detection_score_kernel(const float* __restrict__ x, const int* __restrict__ nb, 
   if (lane == 0) score[warp] = best;
 }
 
+struct DetectionWs {
+  int* start;
+  unsigned* cmax;
+  unsigned char* nonzero;
+};
+
+static size_t detection_layout(int N, int B, void* base, DetectionWs* w_out) {
+  Carver cv(base);
+  DetectionWs w;
+  w.start = cv.take<int>((size_t)B + 1);
+  w.cmax = cv.take<unsigned>(B);
+  w.nonzero = cv.take<unsigned char>((size_t)N + 1);
+  if (w_out != nullptr) *w_out = w;
+  return cv.off;
+}
+
 }  // namespace d3f
 
-extern "C" size_t d3f_detection_scores_workspace_bytes(int N, int B) {
-  return align_up(sizeof(int) * (size_t)(B + 1), 256) + align_up(sizeof(unsigned) * (size_t)B, 256) + align_up((size_t)N + 1, 256);
-}
+extern "C" size_t d3f_detection_scores_workspace_bytes(int N, int B) { return detection_layout(N, B, nullptr, nullptr); }
 
 extern "C" int d3f_detection_scores(const float* feats, const int* neighbors, const int* lengths, int B, int N, int H,
                                     int D, float* out_scores, void* workspace, size_t workspace_bytes,
@@ -275,12 +297,13 @@ extern "C" int d3f_detection_scores(const float* feats, const int* neighbors, co
   D3F_REQUIRE(N == 0 || (feats && (neighbors || H == 0) && lengths && out_scores && workspace), D3F_ERR_INVALID,
               "d3f_detection_scores: null pointer");
   D3F_REQUIRE(B >= 1 && B <= kMaxBatch && N >= 0 && H >= 0 && D >= 1, D3F_ERR_INVALID, "detection_scores: bad shape");
-  D3F_REQUIRE(workspace_bytes >= d3f_detection_scores_workspace_bytes(N, B), D3F_ERR_WORKSPACE, "detection_scores: workspace too small");
+  DetectionWs w;
+  const size_t need = detection_layout(N, B, workspace, &w);
+  D3F_REQUIRE(workspace_bytes >= need, D3F_ERR_WORKSPACE, "detection_scores: workspace too small");
   if (N == 0) return D3F_OK;
-  Carver cv(workspace, workspace_bytes);
-  int* start = cv.take<int>(B + 1);
-  unsigned* cmax = cv.take<unsigned>(B);
-  unsigned char* nonzero = cv.take<unsigned char>((size_t)N + 1);
+  int* start = w.start;
+  unsigned* cmax = w.cmax;
+  unsigned char* nonzero = w.nonzero;
   int rc = launch_batch_start(lengths, B, start, stream);
   if (rc) return rc;
   D3F_CUDA(cudaMemsetAsync(cmax, 0, sizeof(unsigned) * B, stream));

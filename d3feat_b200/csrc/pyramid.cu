@@ -18,14 +18,59 @@ struct GridSlot {
   float radius;
   void* ws;
   size_t bytes;
-};
-
-struct PyramidPlan {
-  int L;
-  const d3f_pyramid_spec* spec;
+  bool built;   // set by the build when it first searches this grid
 };
 
 inline bool same_radius(float a, float b) { return fabsf(a - b) <= 1e-6f * fmaxf(fabsf(a), fabsf(b)); }
+
+struct PyramidWs {
+  void* sub;   // the subsampling workspace, sized for level 0 and reused by every level
+  size_t sub_bytes;
+  int* starts;   // [D3F_MAX_LEVELS][B + 1] exclusive scans of every level's lengths
+  int* counts;   // [D3F_MAX_LEVELS] level row counts, when the caller keeps none
+  int* status;   // [1], when the caller keeps none
+  GridSlot slots[3 * D3F_MAX_LEVELS];   // in build order
+  int n_slots;
+};
+
+// The grids are listed in the order the build first uses them: per level l the conv grid over level l, then, when
+// level l is subsampled into level l + 1, the pool grid over level l and the upsample grid over level l + 1. A grid is
+// keyed by (level, radius) and sized with the row capacity of its level; a radius <= 0 has none.
+size_t pyramid_layout(int B, const d3f_pyramid_spec* spec, const int* capacity, const float* host_bbox, void* base,
+                      PyramidWs* w_out) {
+  if (spec == nullptr || capacity == nullptr || host_bbox == nullptr) return 0;
+  const int L = spec->n_levels;
+  if (L < 1 || L > D3F_MAX_LEVELS) return 0;
+  Carver cv(base);
+  PyramidWs w;
+  w.sub_bytes = d3f_grid_subsample_workspace_bytes(capacity[0], B);
+  w.sub = cv.take<char>(w.sub_bytes);
+  w.starts = cv.take<int>((size_t)D3F_MAX_LEVELS * (B + 1));
+  w.counts = cv.take<int>(D3F_MAX_LEVELS);
+  w.status = cv.take<int>(1);
+  w.n_slots = 0;
+  auto add = [&](int l, float radius) {
+    if (!(radius > 0.f)) return true;
+    for (int i = 0; i < w.n_slots; ++i)
+      if (w.slots[i].level == l && same_radius(w.slots[i].radius, radius)) return true;
+    const size_t nb = d3f_radius_neighbors_workspace_bytes(capacity[l], B, radius, host_bbox);
+    if (nb == 0) return false;
+    GridSlot& g = w.slots[w.n_slots++];
+    g.level = l;
+    g.radius = radius;
+    g.ws = cv.take<char>(nb);
+    g.bytes = nb;
+    g.built = false;
+    return true;
+  };
+  for (int l = 0; l < L; ++l) {
+    if (!add(l, spec->conv_radius[l])) return 0;
+    if (spec->sub_dl[l] > 0.f && l + 1 < L && !(add(l, spec->pool_radius[l]) && add(l + 1, spec->up_radius[l])))
+      return 0;
+  }
+  if (w_out != nullptr) *w_out = w;
+  return cv.off;
+}
 
 }  // namespace
 
@@ -37,29 +82,9 @@ __global__ void set_count_kernel(int* __restrict__ dst, int value, const int* __
 
 using namespace d3f;
 
-// Workspace: one subsampling workspace (level-0 sized) + one grid workspace per distinct (level, radius) pair,
-// sized with the per-level row capacity.
 extern "C" size_t d3f_pyramid_workspace_bytes(int B, const d3f_pyramid_spec* spec, const int* capacity,
                                               const float* host_bbox) {
-  if (spec == nullptr || capacity == nullptr || host_bbox == nullptr) return 0;
-  int L = spec->n_levels;
-  if (L < 1 || L > D3F_MAX_LEVELS) return 0;
-  size_t total = align_up(d3f_grid_subsample_workspace_bytes(capacity[0], B) + 512, 256);
-  total += align_up(sizeof(int) * (size_t)D3F_MAX_LEVELS * (B + 1), 256);   // exclusive scans of every level's lengths
-  for (int l = 0; l < L; ++l) {
-    float radii[3] = {spec->conv_radius[l], spec->sub_dl[l] > 0.f ? spec->pool_radius[l] : -1.f,
-                      (l > 0 && spec->sub_dl[l - 1] > 0.f) ? spec->up_radius[l - 1] : -1.f};
-    for (int a = 0; a < 3; ++a) {
-      if (!(radii[a] > 0.f)) continue;
-      bool dup = false;
-      for (int b = 0; b < a; ++b) dup = dup || (radii[b] > 0.f && same_radius(radii[a], radii[b]));
-      if (dup) continue;
-      size_t nb = d3f_radius_neighbors_workspace_bytes(capacity[l], B, radii[a], host_bbox);
-      if (nb == 0) return 0;
-      total += align_up(nb, 256);
-    }
-  }
-  return total + 1024;
+  return pyramid_layout(B, spec, capacity, host_bbox, nullptr, nullptr);
 }
 
 // Two ways to run it:
@@ -89,29 +114,22 @@ extern "C" int d3f_pyramid_build(const float* points, const int* lengths, int B,
   const int L = spec->n_levels;
   D3F_REQUIRE(L >= 1 && L <= D3F_MAX_LEVELS, D3F_ERR_INVALID, "pyramid_build: n_levels=%d", L);
   D3F_REQUIRE(N0 >= 0 && N0 <= capacity[0], D3F_ERR_CAPACITY, "pyramid_build: N0=%d exceeds capacity %d", N0, capacity[0]);
-  D3F_REQUIRE(workspace_bytes >= d3f_pyramid_workspace_bytes(B, spec, capacity, host_bbox) &&
-                  d3f_pyramid_workspace_bytes(B, spec, capacity, host_bbox) > 0,
-              D3F_ERR_WORKSPACE, "pyramid_build: workspace too small (or grid too large)");
+  PyramidWs w;
+  const size_t need = pyramid_layout(B, spec, capacity, host_bbox, workspace, &w);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE,
+              "pyramid_build: workspace too small (or grid too large)");
 
-  char* base = (char*)workspace;
-  size_t off = 0;
-  void* sub_ws = base;
-  size_t sub_bytes = align_up(d3f_grid_subsample_workspace_bytes(capacity[0], B) + 512, 256);
-  off += sub_bytes;
   // start[l][b] = first row of cloud b at level l: scanned ONCE per level (every grid build, search and subsampling
   // of that level used to launch its own scan: 22 launches per step instead of 5)
-  int* starts = (int*)(base + off);
-  off += align_up(sizeof(int) * (size_t)D3F_MAX_LEVELS * (B + 1), 256);
+  int* starts = w.starts;
   if (launch_batch_start(lengths, B, starts, stream)) return D3F_ERR_CUDA;
-  // level counts live in the caller's buffer, or (exact form without one) in the tail of the subsampling region
-  int* counts = d_counts != nullptr ? d_counts : (int*)((char*)sub_ws + sub_bytes - 256);
-  int* status = d_status != nullptr ? d_status : counts + D3F_MAX_LEVELS;
+  // level counts and status live in the caller's buffers, or (exact form without them) in the workspace
+  int* counts = d_counts != nullptr ? d_counts : w.counts;
+  int* status = d_status != nullptr ? d_status : w.status;
   if (d_status == nullptr) D3F_CUDA(cudaMemsetAsync(status, 0, sizeof(int), stream));
   set_count_kernel<<<1, 1, 0, stream>>>(counts, N0, n0_dev);
   D3F_LAUNCH_CHECK("set_count_kernel");
 
-  GridSlot slots[3 * D3F_MAX_LEVELS];
-  int n_slots = 0;
   const float* lvl_pts[D3F_MAX_LEVELS];
   const int* lvl_len[D3F_MAX_LEVELS];
   int lvl_n[D3F_MAX_LEVELS];   // launch size of level l: exact form = its row count, static form = its capacity
@@ -119,26 +137,19 @@ extern "C" int d3f_pyramid_build(const float* points, const int* lengths, int B,
   lvl_len[0] = lengths;
   lvl_n[0] = exact ? N0 : capacity[0];
 
-  // returns the grid over level `l` at `radius`, building it on first use
+  // returns the grid of the layout over level `l` at `radius`, building it on first use
   auto grid_for = [&](int l, float radius, GridSlot** out) -> int {
-    for (int i = 0; i < n_slots; ++i)
-      if (slots[i].level == l && same_radius(slots[i].radius, radius)) {
-        *out = &slots[i];
-        return D3F_OK;
-      }
-    GridSlot& g = slots[n_slots];
-    g.level = l;
-    g.radius = radius;
-    g.bytes = align_up(d3f_radius_neighbors_workspace_bytes(capacity[l], B, radius, host_bbox), 256);
-    g.ws = base + off;
-    off += g.bytes;
-    D3F_REQUIRE(off <= workspace_bytes, D3F_ERR_WORKSPACE, "pyramid_build: workspace exhausted");
-    int rc = radius_neighbors_build(lvl_pts[l], lvl_len[l], B, lvl_n[l], radius, host_bbox, g.ws, g.bytes, stream,
+    for (int i = 0; i < w.n_slots; ++i) {
+      GridSlot& g = w.slots[i];
+      if (g.level != l || !same_radius(g.radius, radius)) continue;
+      *out = &g;
+      if (g.built) return D3F_OK;
+      g.built = true;
+      return radius_neighbors_build(lvl_pts[l], lvl_len[l], B, lvl_n[l], radius, host_bbox, g.ws, g.bytes, stream,
                                     counts + l, starts + (size_t)l * (B + 1));
-    if (rc) return rc;
-    ++n_slots;
-    *out = &g;
-    return D3F_OK;
+    }
+    d3f::set_error("pyramid_build: radius=%g at level %d must be > 0", (double)radius, l);
+    return D3F_ERR_INVALID;
   };
   // the workspace of a grid is carved with the CAPACITY of its level (the query side re-derives the same layout)
   auto fill = [&](int lq, int ls, GridSlot* g, int lim, int* out) -> int {
@@ -162,7 +173,7 @@ extern "C" int d3f_pyramid_build(const float* points, const int* lengths, int B,
                   "pyramid_build: missing output buffers for level %d", l + 1);
       int* d_M = counts + l + 1;
       int rc = grid_subsample(lvl_pts[l], lvl_len[l], B, lvl_n[l], spec->sub_dl[l], nullptr, 0, nullptr, 0, host_bbox,
-                              out_points[l + 1], nullptr, nullptr, out_lengths[l + 1], d_M, sub_ws, sub_bytes - 256,
+                              out_points[l + 1], nullptr, nullptr, out_lengths[l + 1], d_M, w.sub, w.sub_bytes,
                               stream, counts + l, capacity[l + 1], status, starts + (size_t)l * (B + 1));
       if (rc) return rc;
       if (launch_batch_start(out_lengths[l + 1], B, starts + (size_t)(l + 1) * (B + 1), stream)) return D3F_ERR_CUDA;

@@ -390,8 +390,15 @@ struct Work {
   double* sums;
 };
 
-Work carve(void* workspace, size_t bytes, int P, int T, int V) {
-  Carver cv(workspace, bytes);
+// the sizes the workspace depends on: L, P >= 1, T in [1, 2^24], V in [1, T], P * L * 2 and P * T within int32
+bool sizes_ok(int L, int P, int T, int V) {
+  if (L < 1 || P < 1 || T < 1 || T > (1 << 24) || V < 1 || V > T) return false;
+  return (long long)P * L * 2 <= INT32_MAX && (long long)P * ceil_div(T, 32) * 32 <= INT32_MAX;
+}
+
+size_t work_layout(int L, int P, int T, int V, void* base, Work* w_out) {
+  if (!sizes_ok(L, P, T, V)) return 0;
+  Carver cv(base);
   Work w;
   w.nc_eff = cv.take<int>(P);
   w.n_val = cv.take<int>(P);
@@ -399,7 +406,8 @@ Work carve(void* workspace, size_t bytes, int P, int T, int V) {
   w.list = cv.take<int>((size_t)P * V);
   w.inliers = cv.take<int>((size_t)P * V);
   w.sums = cv.take<double>((size_t)P * V);
-  return w;
+  if (w_out != nullptr) *w_out = w;
+  return cv.off;
 }
 
 template <int N>
@@ -434,22 +442,13 @@ int run(const Rows& rows, const int* count, int B, const int* n_corr, const int*
   return D3F_OK;
 }
 
-// the sizes the workspace depends on: L, P >= 1, T in [1, 2^24], V in [1, T], P * L * 2 and P * T within int32
-bool sizes_ok(int L, int P, int T, int V) {
-  if (L < 1 || P < 1 || T < 1 || T > (1 << 24) || V < 1 || V > T) return false;
-  return (long long)P * L * 2 <= INT32_MAX && (long long)P * ceil_div(T, 32) * 32 <= INT32_MAX;
-}
-
 }  // namespace
 }  // namespace d3f
 
 using namespace d3f;
 
 extern "C" size_t d3f_register_pairs_workspace_bytes(int L, int P, int max_iterations, int max_validation) {
-  if (!sizes_ok(L, P, max_iterations, max_validation)) return 0;
-  const size_t P_ = (size_t)P, V = (size_t)max_validation;
-  return 2 * align_up(sizeof(int) * P_, 256) + align_up(sizeof(unsigned) * P_ * ceil_div(max_iterations, 32), 256) +
-         2 * align_up(sizeof(int) * P_ * V, 256) + align_up(sizeof(double) * P_ * V, 256);
+  return work_layout(L, P, max_iterations, max_validation, nullptr, nullptr);
 }
 
 extern "C" int d3f_register_pairs(const float* points, const int* count, int B, int k, const int* corr,
@@ -475,10 +474,10 @@ extern "C" int d3f_register_pairs(const float* points, const int* count, int B, 
   D3F_REQUIRE(points && count && corr && n_corr && pairs && pose && n_inliers && hypothesis && n_validated &&
                   workspace,
               D3F_ERR_INVALID, "register_pairs: null pointer");
-  const size_t need = d3f_register_pairs_workspace_bytes(L, P, max_iterations, max_validation);
-  D3F_REQUIRE(workspace_bytes >= need, D3F_ERR_WORKSPACE, "register_pairs: workspace too small (%zu < %zu bytes)",
-              workspace_bytes, need);
-  const Work w = carve(workspace, workspace_bytes, P, max_iterations, max_validation);
+  Work w;
+  const size_t need = work_layout(L, P, max_iterations, max_validation, workspace, &w);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE,
+              "register_pairs: workspace too small (%zu < %zu bytes)", workspace_bytes, need);
   const Rows rows{points, corr, k, L};
   const double tau2 = distance * distance;
   const int T = max_iterations, V = max_validation;

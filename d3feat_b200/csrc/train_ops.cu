@@ -36,7 +36,7 @@ struct Csr {
   int *counts, *offs, *scan;
 };
 
-static Csr carve_csr(Carver& cv, int E, int Ns) {
+static Csr take_csr(Carver& cv, int E, int Ns) {
   Csr c;
   c.sb.keys[0] = cv.take<uint64_t>(E);
   c.sb.keys[1] = cv.take<uint64_t>(E);
@@ -173,14 +173,31 @@ __global__ void __launch_bounds__(256) bn_dx_kernel(const float* __restrict__ x,
   }
 }
 
+// Both passes carve the same layout; the forward uses p0 and the two C-vectors (scale, shift), the backward all four.
+struct BatchNormWs {
+  double *p0, *p1;   // [row blocks, C] column partials
+  float *a, *b;      // [C]
+};
+
+static size_t batch_norm_layout(int N, int C, void* base, BatchNormWs* w_out) {
+  if (N < 0 || C < 1) return 0;
+  const size_t nb = (size_t)row_blocks(N) * C;
+  Carver cv(base);
+  BatchNormWs w;
+  w.p0 = cv.take<double>(nb);
+  w.p1 = cv.take<double>(nb);
+  w.a = cv.take<float>(C);
+  w.b = cv.take<float>(C);
+  if (w_out != nullptr) *w_out = w;
+  return cv.off;
+}
+
 }  // namespace d3f
 
 using namespace d3f;
 
 extern "C" size_t d3f_batch_norm_train_workspace_bytes(int N, int C) {
-  if (N < 0 || C < 1) return 0;
-  const size_t nb = (size_t)row_blocks(N) * C;
-  return 2 * align_up(nb * sizeof(double), 256) + 6 * align_up((size_t)C * sizeof(float), 256) + 1024;
+  return batch_norm_layout(N, C, nullptr, nullptr);
 }
 
 extern "C" int d3f_batch_norm_train_forward(const float* x, int N, int C, const float* gamma, const float* beta,
@@ -195,15 +212,14 @@ extern "C" int d3f_batch_norm_train_forward(const float* x, int N, int C, const 
               (double)eps);
   D3F_REQUIRE(beta != nullptr && (gamma == nullptr || (moving_mean && moving_var && mean && invstd)),
               D3F_ERR_INVALID, "batch_norm_train_forward: null pointer");
-  D3F_REQUIRE(workspace_bytes >= d3f_batch_norm_train_workspace_bytes(N, C), D3F_ERR_WORKSPACE,
-              "batch_norm_train_forward: workspace too small");
+  BatchNormWs w;
+  const size_t need = batch_norm_layout(N, C, workspace, &w);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "batch_norm_train_forward: workspace too small");
   if (N == 0) return D3F_OK;   // no batch statistics: the moving statistics stay as they are
   D3F_REQUIRE(x && out && workspace, D3F_ERR_INVALID, "batch_norm_train_forward: null pointer");
-  Carver cv(workspace, workspace_bytes);
   const int nblk = row_blocks(N);
-  double* p0 = cv.take<double>((size_t)nblk * C);
-  float* scale = cv.take<float>(C);
-  float* shift = cv.take<float>(C);
+  double* p0 = w.p0;
+  float *scale = w.a, *shift = w.b;
   const int cb = ceil_div(C, 256);
   if (gamma != nullptr) {
     const dim3 grid(ceil_div(C, 32), nblk);
@@ -234,19 +250,17 @@ extern "C" int d3f_batch_norm_train_backward(const float* x, const float* out, c
               "batch_norm_train_backward: bad shape N=%d C=%d", N, C);
   D3F_REQUIRE(gamma != nullptr || dgamma == nullptr, D3F_ERR_INVALID,
               "batch_norm_train_backward: dgamma without gamma (use_batch_norm = False has no gamma)");
-  D3F_REQUIRE(workspace_bytes >= d3f_batch_norm_train_workspace_bytes(N, C), D3F_ERR_WORKSPACE,
-              "batch_norm_train_backward: workspace too small");
+  BatchNormWs w;
+  const size_t need = batch_norm_layout(N, C, workspace, &w);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "batch_norm_train_backward: workspace too small");
   if (dgamma) D3F_CUDA(cudaMemsetAsync(dgamma, 0, (size_t)C * sizeof(float), stream));
   if (dbeta) D3F_CUDA(cudaMemsetAsync(dbeta, 0, (size_t)C * sizeof(float), stream));
   if (N == 0) return D3F_OK;
   D3F_REQUIRE(x && out && dout && workspace && (gamma == nullptr || (mean && invstd)), D3F_ERR_INVALID,
               "batch_norm_train_backward: null pointer");
-  Carver cv(workspace, workspace_bytes);
   const int nblk = row_blocks(N);
-  double* p0 = cv.take<double>((size_t)nblk * C);
-  double* p1 = cv.take<double>((size_t)nblk * C);
-  float* a = cv.take<float>(C);
-  float* b = cv.take<float>(C);
+  double *p0 = w.p0, *p1 = w.p1;
+  float *a = w.a, *b = w.b;
   const dim3 grid(ceil_div(C, 32), nblk);
   colsum_partial_kernel<kColBnGrad><<<grid, 1024, 0, stream>>>(x, out, dout, N, C, mean, invstd, alpha, p0, p1);
   D3F_LAUNCH_CHECK("colsum_partial_kernel");
@@ -380,24 +394,24 @@ struct MaxPoolBwd {
   double* partial;
 };
 
-static MaxPoolBwd carve_maxpool(Carver& cv, int N1, int N2, int H, int C) {
+static size_t maxpool_backward_layout(int N1, int N2, int H, int C, void* base, MaxPoolBwd* w_out) {
+  if (N1 < 1 || N2 < 0 || H < 0 || C < 1 || (long long)N2 * H >= (1ll << 31)) return 0;
+  Carver cv(base);
   MaxPoolBwd w;
-  w.csr = carve_csr(cv, N2 * H, N1);
+  w.csr = take_csr(cv, N2 * H, N1);
   w.cmin = cv.take<unsigned>(C);
   w.nmin = cv.take<int>(C);
   w.gs = cv.take<float>((size_t)N2 * C);
   w.share = cv.take<float>(C);
   w.partial = cv.take<double>((size_t)row_blocks((long long)N2 * H) * C);
-  return w;
+  if (w_out != nullptr) *w_out = w;
+  return cv.off;
 }
 
 }  // namespace d3f
 
 extern "C" size_t d3f_ind_max_pool_backward_workspace_bytes(int N1, int N2, int H, int C) {
-  if (N1 < 1 || N2 < 0 || H < 0 || C < 1 || (long long)N2 * H >= (1ll << 31)) return 0;
-  Carver cv(nullptr, 0);
-  carve_maxpool(cv, N1, N2, H, C);
-  return cv.off + 1024;
+  return maxpool_backward_layout(N1, N2, H, C, nullptr, nullptr);
 }
 
 extern "C" int d3f_ind_max_pool_backward(const float* x, const int* inds, const float* out, const float* dout, int N1,
@@ -410,14 +424,13 @@ extern "C" int d3f_ind_max_pool_backward(const float* x, const int* inds, const 
               "ind_max_pool_backward: N2*H, N2*C or N1*C beyond int32");
   D3F_REQUIRE(x && dx && (N2 == 0 || (inds && out && dout && workspace)), D3F_ERR_INVALID,
               "ind_max_pool_backward: null pointer");
-  D3F_REQUIRE(workspace_bytes >= d3f_ind_max_pool_backward_workspace_bytes(N1, N2, H, C), D3F_ERR_WORKSPACE,
-              "ind_max_pool_backward: workspace too small");
+  MaxPoolBwd w;
+  const size_t need = maxpool_backward_layout(N1, N2, H, C, workspace, &w);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "ind_max_pool_backward: workspace too small");
   if (N2 == 0 || H == 0) {   // nothing was pooled (H = 0: every pooled row is the column minimum of no entry)
     D3F_CUDA(cudaMemsetAsync(dx, 0, (size_t)N1 * C * sizeof(float), stream));
     return D3F_OK;
   }
-  Carver cv(workspace, workspace_bytes);
-  MaxPoolBwd w = carve_maxpool(cv, N1, N2, H, C);
   const int E = N2 * H;
   D3F_CUDA(cudaMemsetAsync(w.cmin, 0xff, (size_t)C * sizeof(unsigned), stream));
   D3F_CUDA(cudaMemsetAsync(w.nmin, 0, (size_t)C * sizeof(int), stream));
@@ -462,13 +475,18 @@ __global__ void __launch_bounds__(256) gather_rows_grad_kernel(const float* __re
   }
 }
 
+static size_t gather_rows_backward_layout(int N1, int N2, void* base, Csr* w_out) {
+  if (N1 < 0 || N2 < 0) return 0;
+  Carver cv(base);
+  const Csr w = take_csr(cv, N2, N1);
+  if (w_out != nullptr) *w_out = w;
+  return cv.off;
+}
+
 }  // namespace d3f
 
 extern "C" size_t d3f_gather_rows_backward_workspace_bytes(int N1, int N2) {
-  if (N1 < 0 || N2 < 0) return 0;
-  Carver cv(nullptr, 0);
-  carve_csr(cv, N2, N1);
-  return cv.off + 1024;
+  return gather_rows_backward_layout(N1, N2, nullptr, nullptr);
 }
 
 extern "C" int d3f_gather_rows_backward(const int* inds, const float* dout, int N1, int N2, int C, float* dx,
@@ -479,15 +497,14 @@ extern "C" int d3f_gather_rows_backward(const int* inds, const float* dout, int 
   D3F_REQUIRE(N1 == 0 || dx, D3F_ERR_INVALID, "gather_rows_backward: null pointer");
   D3F_REQUIRE(N1 == 0 || N2 == 0 || (inds && dout && workspace), D3F_ERR_INVALID,
               "gather_rows_backward: null pointer");
-  D3F_REQUIRE(workspace_bytes >= d3f_gather_rows_backward_workspace_bytes(N1, N2), D3F_ERR_WORKSPACE,
-              "gather_rows_backward: workspace too small");
+  Csr csr;
+  const size_t need = gather_rows_backward_layout(N1, N2, workspace, &csr);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "gather_rows_backward: workspace too small");
   if (N1 == 0) return D3F_OK;
   if (N2 == 0) {
     D3F_CUDA(cudaMemsetAsync(dx, 0, (size_t)N1 * C * sizeof(float), stream));
     return D3F_OK;
   }
-  Carver cv(workspace, workspace_bytes);
-  Csr csr = carve_csr(cv, N2, N1);
   const uint32_t* sorted_q = nullptr;
   int rc = reverse_csr(inds, N2, N1, 1, nullptr, nullptr, csr.sb, csr.counts, csr.offs, csr.scan, &sorted_q, stream);
   if (rc) return rc;
@@ -748,9 +765,11 @@ struct DetBwd {
   unsigned char* nz;
 };
 
-static DetBwd carve_det(Carver& cv, int N, int H, int B, int D) {
+static size_t detection_backward_layout(int N, int H, int B, int D, void* base, DetBwd* w_out) {
+  if (N < 0 || H < 0 || B < 1 || D < 1 || (long long)N * H >= (1ll << 31)) return 0;
+  Carver cv(base);
   DetBwd w;
-  w.csr = carve_csr(cv, N * H, N);
+  w.csr = take_csr(cv, N * H, N);
   w.start = cv.take<int>((size_t)B + 1);
   w.tm = cv.take<int>(B);
   w.cmax = cv.take<unsigned>(B);
@@ -762,16 +781,14 @@ static DetBwd carve_det(Carver& cv, int N, int H, int B, int D) {
   w.A = cv.take<float>(ND);
   w.ginv = cv.take<float>(N);
   w.nz = cv.take<unsigned char>((size_t)N + 1);
-  return w;
+  if (w_out != nullptr) *w_out = w;
+  return cv.off;
 }
 
 }  // namespace d3f
 
 extern "C" size_t d3f_detection_scores_backward_workspace_bytes(int N, int H, int B, int D) {
-  if (N < 0 || H < 0 || B < 1 || D < 1 || (long long)N * H >= (1ll << 31)) return 0;
-  Carver cv(nullptr, 0);
-  carve_det(cv, N, H, B, D);
-  return cv.off + 1024;
+  return detection_backward_layout(N, H, B, D, nullptr, nullptr);
 }
 
 extern "C" int d3f_detection_scores_backward(const float* feats, const int* neighbors, const int* lengths,
@@ -782,13 +799,12 @@ extern "C" int d3f_detection_scores_backward(const float* feats, const int* neig
               "detection_scores_backward: bad shape B=%d N=%d H=%d D=%d", B, N, H, D);
   D3F_REQUIRE((long long)N * max(H, D) < (1ll << 31), D3F_ERR_INVALID,
               "detection_scores_backward: N*H or N*D beyond int32");
-  D3F_REQUIRE(workspace_bytes >= d3f_detection_scores_backward_workspace_bytes(N, H, B, D), D3F_ERR_WORKSPACE,
-              "detection_scores_backward: workspace too small");
+  DetBwd w;
+  const size_t need = detection_backward_layout(N, H, B, D, workspace, &w);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "detection_scores_backward: workspace too small");
   if (N == 0) return D3F_OK;
   D3F_REQUIRE(feats && (neighbors || H == 0) && lengths && dscores && dfeats && workspace, D3F_ERR_INVALID,
               "detection_scores_backward: null pointer");
-  Carver cv(workspace, workspace_bytes);
-  DetBwd w = carve_det(cv, N, H, B, D);
   int rc = launch_batch_start(lengths, B, w.start, stream);
   if (rc) return rc;
   D3F_CUDA(cudaMemsetAsync(w.cmax, 0, sizeof(unsigned) * B, stream));

@@ -168,8 +168,11 @@ struct VoxelWs {
   int* total;
 };
 
-static size_t carve_voxel(Carver& cv, int N, int B, VoxelWs& w) {
+static size_t voxel_layout(int N, int B, void* base, VoxelWs* w_out) {
+  if (N < 0 || B < 1 || B > kMaxBatch) return 0;
   const int n = N > 0 ? N : 1;
+  Carver cv(base);
+  VoxelWs w;
   w.sort.keys[0] = cv.take<uint64_t>(n);
   w.sort.keys[1] = cv.take<uint64_t>(n);
   w.sort.vals[0] = cv.take<uint32_t>(n);
@@ -183,6 +186,7 @@ static size_t carve_voxel(Carver& cv, int N, int B, VoxelWs& w) {
   w.err = cv.take<int>(1);
   w.n_rows = cv.take<int>(1);
   w.total = cv.take<int>(1);
+  if (w_out != nullptr) *w_out = w;
   return cv.off;
 }
 
@@ -190,12 +194,7 @@ static size_t carve_voxel(Carver& cv, int N, int B, VoxelWs& w) {
 
 using namespace d3f;
 
-extern "C" size_t d3f_voxel_down_sample_workspace_bytes(int N, int B) {
-  if (N < 0 || B < 1 || B > kMaxBatch) return 0;
-  Carver cv(nullptr, ~(size_t)0);
-  VoxelWs w;
-  return carve_voxel(cv, N, B, w) + 256;
-}
+extern "C" size_t d3f_voxel_down_sample_workspace_bytes(int N, int B) { return voxel_layout(N, B, nullptr, nullptr); }
 
 extern "C" int d3f_voxel_down_sample(const float* pts, const int* lengths, int B, int N, const int* n_dev,
                                      double voxel_size, const float* host_bbox, float* out_pts, int* out_lengths,
@@ -214,8 +213,9 @@ extern "C" int d3f_voxel_down_sample(const float* pts, const int* lengths, int B
   for (int a = 0; a < 6; ++a)
     D3F_REQUIRE(isfinite(host_bbox[a]), D3F_ERR_INVALID, "voxel_down_sample: host_bbox[%d]=%g is not finite", a,
                 (double)host_bbox[a]);
-  D3F_REQUIRE(workspace_bytes >= d3f_voxel_down_sample_workspace_bytes(N, B), D3F_ERR_WORKSPACE,
-              "voxel_down_sample: workspace too small");
+  VoxelWs w;
+  const size_t need = voxel_layout(N, B, workspace, &w);
+  D3F_REQUIRE(need > 0 && workspace_bytes >= need, D3F_ERR_WORKSPACE, "voxel_down_sample: workspace too small");
   VoxelBits bits;
   bits.x = voxel_axis_bits((double)host_bbox[3] - (double)host_bbox[0], voxel_size);
   bits.y = voxel_axis_bits((double)host_bbox[4] - (double)host_bbox[1], voxel_size);
@@ -228,9 +228,6 @@ extern "C" int d3f_voxel_down_sample(const float* pts, const int* lengths, int B
               D3F_ERR_CAPACITY, "voxel_down_sample: a grid of 2^%d x 2^%d x 2^%d voxels x %d clouds exceeds the sort key",
               bits.x, bits.y, bits.z, B);
 
-  Carver cv(workspace, workspace_bytes);
-  VoxelWs w;
-  carve_voxel(cv, N, B, w);
   D3F_CUDA(cudaMemsetAsync(out_lengths, 0, sizeof(int) * B, stream));
   if (N == 0) {
     D3F_CUDA(cudaMemsetAsync(out_M, 0, sizeof(int), stream));

@@ -176,7 +176,8 @@ int d3f_radius_neighbors_count(const float* queries, const int* q_batch_len, int
                                int* counts, int* out_max, d3f_stream_t stream);
 /* out_order[Ns]: the support indices in hash-grid cell order (a spatially coherent visiting order). Passing it
  * as `query_order` to d3f_kpconv_forward when queries == supports makes neighbouring queries share their
- * gathered rows in L1/L2; results are unchanged (each query still writes its own output row). */
+ * gathered rows in L1/L2; results are unchanged (each query still writes its own output row). Arguments whose grid
+ * d3f_radius_neighbors_build refuses give D3F_ERR_INVALID (no such workspace can have been built). */
 int d3f_radius_neighbors_order(const void* workspace, int Ns, int B, float radius,
                                const float* host_bbox, int* out_order, d3f_stream_t stream);
 int d3f_radius_neighbors_fill(const float* queries, const int* q_batch_len, int Nq,
@@ -318,7 +319,7 @@ int d3f_unary_backward(const float* x, const float* W, const float* dout, int N,
                        const int* n_dev);
 
 /* out[N2,C] = max_h x'[inds[n,h]] with x' = x || colmin(x) (shadow index = N1).
- * workspace: C floats. */
+ * workspace: C + 1 unsigned words (the ordered column minima and a flag). */
 size_t d3f_ind_max_pool_workspace_bytes(int C);
 int d3f_ind_max_pool(const float* x, const int* inds, int N1, int N2, int H, int C, float* out,
                      void* workspace, size_t workspace_bytes, d3f_stream_t stream, const int* n1_dev,
